@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the NeuMesh rendering hot path on B200.
+"""Benchmark of the NeuMesh rendering hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...   # the reference algorithm's CPU path (oracle port)
@@ -7,6 +7,9 @@
 One step = one 800x800 frame of the synthetic spiral (640 000 rays, the configuration BASELINE.json's metric is quoted
 on: icosphere mesh V = 163 842, 32-d vertex codes, K = 8, calc_normal + white background, bounded near/far, 64 + 64
 samples).  Prints ONE JSON line (rank 0).  Keys are documented in DESIGN.md "Measurement".
+
+``--dump-outputs DIR`` writes what the timed path returned for its last step (``DIR/<name>.npy``, float32) so that two
+builds can be compared output for output: the inputs depend only on the arguments.
 """
 from __future__ import annotations
 
@@ -34,8 +37,8 @@ DEFAULT_ENGINE = "tcgen05_f16"
 CODE_DIM = 32
 WORKLOAD_NAME = "spiral_800x800_icosphere_V163842_F32_K8"
 
-# BASELINE.json configs as bench workloads.  The default (and the only one the driver times) is the configuration the
-# headline metric is quoted on; the others are for `python bench.py --workload ...` measurements recorded in profiles/.
+# BASELINE.json configs as bench workloads.  The default is the configuration the headline metric is quoted on; the
+# others are for `python bench.py --workload ...` measurements.
 WORKLOADS = {
     "spiral800": dict(H=800, W=800, level=7, code=32, kw=RENDER_KW, name="spiral_800x800_icosphere_V163842_F32_K8"),
     # config 2: "DTU scan63 full-res spiral" = 1600 x 1200 frames of the same scene
@@ -70,8 +73,8 @@ BYTES_KNN = 12 + 8 * 24                                   # 204 B per KNN query 
 
 
 def host_cores():
-    """Physical cores of the host: MKL / OpenMP run the oracle fastest at one thread per physical core (measured on the
-    GPU box: 210 rays/s at 64 threads, 39-50 rays/s at 128 hyper-threads)."""
+    """Physical cores of the host: MKL / OpenMP run the oracle fastest at one thread per physical core (hyper-threads
+    slow it down)."""
     try:
         import psutil
         n = psutil.cpu_count(logical=False)
@@ -92,11 +95,12 @@ def measured_peaks():
                     "source": "measured"}
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s - not reached figures
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -219,13 +223,33 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out, path):
+    """The arrays of one step's output dict -> ``path/<name>.npy`` (float32).  Above DUMP_LIMIT_BYTES in all, every array
+    keeps the same fixed, seeded sample of the rays, and ``ray_index.npy`` (float64) says which."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: v.detach().float().cpu() for k, v in out.items() if torch.is_tensor(v) and v.numel()}
+    n = min(v.shape[0] for v in arrays.values())
+    total = sum(v.numel() * 4 for v in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        keep = max(1, int(n * DUMP_LIMIT_BYTES // total) - 1)
+        idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        arrays = {k: v[idx] for k, v in arrays.items()}
+        np.save(os.path.join(path, "ray_index.npy"), idx.double().numpy())
+    for k, v in arrays.items():
+        np.save(os.path.join(path, k + ".npy"), v.numpy())
+
+
 def workload_config(rays_per_step):
     return {"workload": WORKLOAD_NAME, "image": [H, W], "rays_per_step": rays_per_step,
             "mesh_vertices": 10 * 4 ** MESH_LEVEL + 2, "vertex_code_dim": CODE_DIM, "knn_k": 8,
             "N_samples": RENDER_KW.get("N_samples", 64), "N_importance": RENDER_KW.get("N_importance", 64),
             "render": RENDER_KW,
             "l2": "inputs larger than L2: every step renders a different spiral view and streams ~12 GB of per-sample "
-                  "scratch per frame (126 MB L2)"}
+                  "scratch per frame (50 MB L2)"}
 
 
 def main():
@@ -237,7 +261,7 @@ def main():
     ap.add_argument("--engine", default=DEFAULT_ENGINE, choices=["tcgen05", "fp32", "tcgen05_f16"],
                     help="MLP engine: tcgen05_f16 = fp16x3 operands (default), tcgen05 = 3xTF32, fp32 = CUDA cores")
     ap.add_argument("--workload", default="spiral800", choices=sorted(WORKLOADS) + ["train"],
-                    help="spiral800 = the headline configuration (default, the one the driver times); scan63_full / "
+                    help="spiral800 = the headline configuration (default); scan63_full / "
                          "codes256 / big = BASELINE configs 2 / 3 / 5; train = config 4 (512 rays per GPU per step)")
     ap.add_argument("--image", type=int, default=0, help="override the (square) image size of the workload")
     ap.add_argument("--shard", default="auto", choices=["auto", "frame", "rays"],
@@ -256,7 +280,14 @@ def main():
     ap.add_argument("--all-samples", action="store_true",
                     help="evaluate colour / nabla at every sample like the reference does, instead of only where the "
                          "visibility weight is non-zero (bit-identical outputs either way)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy (float32; a fixed "
+                         "seeded sample of the rays when they exceed 64 MB)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload == "train" or args.impl == "reference" or args.simulate_world > 1 or args.tune
+                              or args.steps < 1):
+        ap.error("--dump-outputs needs at least one timed step of the rendering path (not --workload train, "
+                 "--impl reference, --simulate-world or --tune)")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -295,8 +326,8 @@ def main():
     model = model.to(dev).eval()
     n_rays = H * W * fps                             # rays per step: `fps` consecutive spiral frames, pooled
     # partition of a step over the ranks: whole frames when there is at least one per rank (a rank's Morton-ordered
-    # rays then belong to ONE camera pose - pooling blocks of eight different poses made the per-rank octree walks 30 %
-    # slower at 8 GPUs in round 1), block-cyclic blocks of 128 rays otherwise (single-frame latency mode)
+    # rays then belong to ONE camera pose - pooling blocks of different poses slows the per-rank octree walks),
+    # block-cyclic blocks of 128 rays otherwise (single-frame latency mode)
     by_frame = (args.shard == "frame" or (args.shard == "auto" and fps % world == 0 and fps >= world)) and sim == 1 \
         and world > 1 and fps % world == 0
     if by_frame:
@@ -375,6 +406,8 @@ def main():
         launches = _lib.launch_count() - launches0
         prof = _lib.profile_collect()
         _lib.profile_enable(False)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(out, args.dump_outputs)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         ms_total = float(ms.item())
@@ -430,6 +463,7 @@ def main():
 
     if rank == 0:
         peaks = measured_peaks()
+        props = torch.cuda.get_device_properties(dev)
         value = n_rays * args.steps / (ms_total * 1e-3)
         e2e_val = n_rays * args.steps / (ms_e2e * 1e-3)
         # ---- per-kernel-class device time of THIS rank over the timed region ----
@@ -447,7 +481,7 @@ def main():
                 kern[k]["gbs_algorithmic"] = kern[k]["points_per_step"] * BYTES_KNN / (kern[k]["ms_per_step"] * 1e-3) / 1e9
         mlp = [k for k in ("geo", "geo_jvp", "color") if k in kern]
         walk = [k for k in ("knn", "knn_list", "bound_scan") if k in kern]
-        if mlp:   # the three instantiations of the ONE tcgen05 kernel template, taken together
+        if mlp:   # the three instantiations of the ONE MLP kernel template, taken together
             tot_ms = sum(kern[k]["ms_per_step"] for k in mlp)
             tot_fl = sum(kern[k]["points_per_step"] * flops[k] for k in mlp)
             kern["mlp_tc"] = {"ms_per_step": tot_ms, "launches_per_step": sum(kern[k]["launches_per_step"] for k in mlp),
@@ -455,7 +489,7 @@ def main():
                               "tflops_algorithmic": tot_fl / (tot_ms * 1e-3) / 1e12}
             mlp = mlp + ["mlp_tc"]
         kname = {"geo": "mlp_tc_kernel<0> (geometry MLP)", "geo_jvp": "mlp_tc_kernel<1> (geometry MLP + tangent rows)",
-                 "color": "mlp_tc_kernel<2> (colour MLP)", "mlp_tc": "mlp_tc_kernel<0|1|2> (tcgen05 field MLPs, all "
+                 "color": "mlp_tc_kernel<2> (colour MLP)", "mlp_tc": "mlp_tc_kernel<0|1|2> (wgmma field MLPs, all "
                  "instantiations)", "knn": "knn_rays_kernel (8-NN walk + mesh distance, ray-ordered)",
                  "knn_list": "knn_lists_kernel (8-NN walk + mesh distance, live samples)",
                  "bound_scan": "bound_dir_kernel<false|true> (bounded near/far: front-to-back + back-to-front scans)"}
@@ -463,13 +497,12 @@ def main():
         def tensor_roofline(k):
             peak = peaks["bf16_tflops_sustained"]
             ach = kern[k]["tflops_algorithmic"]
-            split = ("every MAC is issued 3x as kind::f16 (fp16x3 split operands, fp32-accurate; needed for the 1e-4 / 1e-5 "
-                     "parity bar), so the ceiling of this fraction is 1/3" if args.engine == "tcgen05_f16" else
-                     "every MAC is issued 3x as kind::tf32 (3xTF32 split) and TF32 runs at half the bf16 rate, so the "
+            split = ("every MAC is issued 3x as fp16 wgmma (fp16x3 split operands, fp32-accurate; needed for the 1e-4 / "
+                     "1e-5 parity bar), so the ceiling of this fraction is 1/3" if args.engine == "tcgen05_f16" else
+                     "every MAC is issued 3x as tf32 wgmma (3xTF32 split) and TF32 runs at half the bf16 rate, so the "
                      "ceiling of this fraction is 1/6")
             return {"bound": "tensor", "kernel": kname[k], "achieved": ach, "peak": peak, "unit": "TFLOP/s",
-                    "frac": ach / peak, "traffic": traffic_of(k),
-                    "peak_source": f"{peaks['source']} dense bf16 cuBLAS, sustained",
+                    "frac": ach / peak, "peak_source": f"{peaks['source']}, dense bf16",
                     "avg_launch_ms": kern[k]["ms_per_step"] / kern[k]["launches_per_step"],
                     "ms_per_step": kern[k]["ms_per_step"],
                     "note": "achieved = algorithmic fp32-equivalent FLOPs (each MAC once, reference dims) / device time "
@@ -478,42 +511,13 @@ def main():
         def hbm_roofline(k):
             ach = kern[k]["gbs_algorithmic"]
             return {"bound": "hbm", "kernel": kname[k], "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                    "frac": ach / peaks["hbm_gbs"], "traffic": traffic_of(k),
-                    "peak_source": f"{peaks['source']} copy bandwidth",
+                    "frac": ach / peaks["hbm_gbs"], "peak_source": f"{peaks['source']}, HBM bandwidth",
                     "avg_launch_ms": kern[k]["ms_per_step"] / kern[k]["launches_per_step"],
                     "ms_per_step": kern[k]["ms_per_step"],
                     "note": "achieved = 204 algorithmic bytes per query (xyz + 8 x (vertex + indicator)) x queries / "
                             "device time.  The octree index (5.9 MB) is L2-resident and the walk is a divergent, "
-                            "latency-bound pointer chase (ncu: DRAM < 1 %, SIMT efficiency 6-8 of 32 lanes, "
-                            "long_scoreboard dominant): HBM bandwidth is the nominal roofline for a gather, not the "
+                            "latency-bound pointer chase: HBM bandwidth is the nominal roofline for a gather, not the "
                             "binding limit here"}
-
-        traffic_tab = {}
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            try:
-                traffic_tab = json.load(open(tpath))
-            except Exception:
-                traffic_tab = {}
-
-        def traffic_of(k):
-            """DRAM bytes per launch: ncu-measured bytes per processed point x points per launch of this run."""
-            tab = traffic_tab.get("bytes_per_point", {})
-            if k == "mlp_tc":
-                parts = [kk for kk in ("geo", "geo_jvp", "color") if kk in kern and kk in tab]
-                if not parts:
-                    return None
-                return sum(tab[kk] * kern[kk]["points_per_step"] for kk in parts) / kern[k]["launches_per_step"]
-            if k == "walk":
-                parts = [kk for kk in ("knn", "knn_list", "bound_scan") if kk in kern]
-                vals = [traffic_of(kk) for kk in parts]
-                if any(v is None for v in vals):
-                    return None
-                return sum(v * kern[kk]["launches_per_step"] for v, kk in zip(vals, parts)) / kern[k]["launches_per_step"]
-            bpp = tab.get("knn" if k == "knn_list" else k)
-            if bpp is None or k not in kern or not kern[k]["launches_per_step"]:
-                return None
-            return bpp * kern[k]["points_per_step"] / kern[k]["launches_per_step"]
 
         if walk:   # the three octree-walk kernels share knn_walk.cuh: one class, like the MLP instantiations
             tot_ms = sum(kern[k]["ms_per_step"] for k in walk)
@@ -526,7 +530,7 @@ def main():
         secondary = None
         allk = mlp + walk
         if allk:
-            # the two kernel CLASSES of the frame: every tcgen05 MLP instantiation together, every octree walk together
+            # the two kernel CLASSES of the frame: every MLP instantiation together, every octree walk together
             cls = [k for k in ("mlp_tc", "walk") if k in kern]
             cls.sort(key=lambda k: -kern[k]["ms_per_step"])
             mk = lambda k: tensor_roofline(k) if k in mlp else hbm_roofline(k)   # noqa: E731
@@ -535,27 +539,6 @@ def main():
             roofline["by_class"] = {k: mk(k) for k in allk}
             for v in roofline["by_class"].values():
                 v.pop("note", None)
-            walk_issue = traffic_tab.get("walk_issue")
-            if walk_issue and "walk" in kern:
-                # honest second roofline of the latency / issue-bound walks: warp instructions per query from the ncu
-                # capture of this very kernel x queries per second, against the SMs' issue rate at the sampled clock
-                sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-                # queries that are really walked: the ray-ordered and the live-list kernels (the bound scan's nominal
-                # 256 samples per ray are mostly decided by the certificate grid without a walk)
-                qk = [k for k in ("knn", "knn_list") if k in kern]
-                qps = sum(kern[k]["points_per_step"] for k in qk) / (sum(kern[k]["ms_per_step"] for k in qk) * 1e-3)
-                peak = 148 * 4 * sm_mhz * 1e6
-                tgt = roofline if cls[0] == "walk" else secondary
-                tgt["issue_slots"] = {"warp_inst_per_query": walk_issue["warp_inst_per_query"],
-                                      "active_lanes_per_inst": walk_issue["active_lanes_per_inst"],
-                                      "achieved_warp_inst_per_s": qps * walk_issue["warp_inst_per_query"],
-                                      "peak_warp_inst_per_s": peak,
-                                      "frac": qps * walk_issue["warp_inst_per_query"] / peak,
-                                      "kernels": "knn_rays_kernel + knn_lists_kernel",
-                                      "note": "share of the SMs' warp-instruction issue slots the walks use (ncu "
-                                              "issue-active 68-72 %); only ~10 of 32 lanes are active per issued "
-                                              "instruction, so the USEFUL fraction is ~0.3 x this",
-                                      "source": walk_issue.get("source", "profiles/")}
         cpu = None
         if world == 1 and args.cpu_rays > 0:
             rate, secs = cpu_oracle_rate(cfg, mesh, sd, frames[0][0], frames[0][1], args.cpu_rays)
@@ -568,8 +551,8 @@ def main():
             "metric": METRIC, "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_total / args.steps, "higher_is_better": True,
             "scaling": scaling, "vs_baseline": None,
-            "dtype": {"tcgen05": "fp32 (MLPs: 3xTF32 tcgen05, fp32 accumulate)",
-                      "tcgen05_f16": "fp32 (MLPs: fp16x3 split operands on tcgen05 kind::f16, fp32 accumulate; sdf error "
+            "dtype": {"tcgen05": "fp32 (MLPs: 3xTF32 wgmma, fp32 accumulate)",
+                      "tcgen05_f16": "fp32 (MLPs: fp16x3 split operands on fp16 wgmma, fp32 accumulate; sdf error "
                                      "vs float64 equal to plain fp32)"}.get(args.engine, "fp32"),
             "data": "synthetic", "config": {**workload_config(n_rays), "frames_per_step": fps,
                                             "parallelism": (f"whole-frame shard x{world} + all_gather" if by_frame else
@@ -579,6 +562,7 @@ def main():
             "e2e": {"value": e2e_val, "unit": "rays/s", "ms_per_step": ms_e2e / args.steps,
                     "h2d_bytes_per_step": bo, "d2h_bytes_per_step": bi,
                     "api": "neumesh_b200.volume_render on pinned host rays; rgb + depth read back to pinned host"},
+            "gpu": {"name": torch.cuda.get_device_name(dev), "sm_count": props.multi_processor_count},
             "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "roofline_secondary": secondary,
             "kernels": kern,
             "all_samples": {"value": n_rays * args.steps / (ms_all * 1e-3), "unit": "rays/s",

@@ -176,7 +176,7 @@ def main(args, rank, world, local_rank):
         line = {"metric": "train_rays_per_sec_512_rays_per_gpu", "value": rays / (ms.item() * 1e-3), "unit": "rays/s",
                 "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms.item() / args.steps,
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": "fp32 (training kernels: fp32 FFMA; sampling cascade: fp16x3 / 3xTF32 tcgen05)",
+                "dtype": "fp32 (training kernels: fp32 FFMA; sampling cascade: fp16x3 / 3xTF32 wgmma)",
                 "data": "synthetic",
                 "config": {"workload": "train_step_icosphere_V163842_F32_K8_512rays_per_gpu", "rays_per_gpu": N_RAYS,
                            "points_per_gpu_per_step": pts, "render": KW, "optimizer": "Adam",

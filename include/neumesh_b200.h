@@ -1,5 +1,5 @@
 /*
- * neumesh_b200 - C ABI of the B200-native NeuMesh rendering hot path.
+ * neumesh_b200 - C ABI of the Hopper-native (sm_90a) NeuMesh rendering hot path.
  *
  * The reference (zju3dv/NeuMesh) is pure Python: it has no FFI of its own.  Its only native code on this path is
  * the third-party `frnn` extension, reached through `frnn.frnn_grid_points` at models/mesh_grid.py:64 and :109.
@@ -92,9 +92,8 @@ typedef struct nmb_field_desc {
   const float* col_b[8];
 } nmb_field_desc;
 
-/* mlp_engine: 0 = tcgen05 3xTF32 tensor-core MLP (default), 1 = fp32 FFMA MLP (verification path),
- * 2 = tcgen05 fp16x3 tensor-core MLP (EXPERIMENTAL: fp16 hi/lo operands, weights packed as 2^8 W; same accuracy in the
- * CPU emulation of tools/split_precision_study.py, not yet validated on hardware - never selected by default) */
+/* mlp_engine: 0 = wgmma 3xTF32 tensor-core MLP, 1 = fp32 FFMA MLP (verification path),
+ * 2 = wgmma fp16x3 tensor-core MLP (fp16 hi/lo operands, weights packed as 2^8 W; the Python layer's default engine) */
 int nmb_field_create(const nmb_grid* g, const nmb_field_desc* desc, int mlp_engine, void* stream, nmb_field** out);
 void nmb_field_destroy(nmb_field* f);
 /* re-pack after the caller changed parameter values in place (same shapes) */

@@ -1,4 +1,4 @@
-"""neumesh_b200 - B200-native implementation of the NeuMesh volumetric-rendering hot path.
+"""neumesh_b200 - Hopper-native (H100, sm_90a) implementation of the NeuMesh volumetric-rendering hot path.
 
 Public surface (mirrors the reference's Python API for this path):
 
@@ -9,7 +9,7 @@ Public surface (mirrors the reference's Python API for this path):
 * ``TextureEditableNeuMesh`` <- editing/texture_neumesh/texture_neumesh.py
 * ``parallel.render_sharded`` <- the ``nn.DataParallel`` ray scatter / gather of models/trainer.py:39-42
 
-The compute lives in ``lib/libneumesh_b200.so`` (hand-written sm_100a CUDA behind the C ABI of
+The compute lives in ``lib/libneumesh_b200.so`` (hand-written sm_90a CUDA behind the C ABI of
 ``include/neumesh_b200.h``); importing this package does not load it, using it does - and fails loudly if the
 extension is missing: there is no CPU fallback.
 """

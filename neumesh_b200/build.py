@@ -1,4 +1,4 @@
-"""Build ``libneumesh_b200.so`` (hand-written sm_100a CUDA behind a C ABI) and the oracle's C helpers, in-tree.
+"""Build ``libneumesh_b200.so`` (hand-written sm_90a CUDA behind a C ABI) and the oracle's C helpers, in-tree.
 
 ``python -m neumesh_b200.build`` or ``__graft_entry__.build()``.  nvcc cross-compiles without a GPU.
 """
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libneumesh_b200.so")
 SOURCES = ["api.cu", "grid.cu", "field.cu", "field_ffma.cu", "field_tc.cu", "render.cu", "shell.cu", "train.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr"]
 
 
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     if force or _newer(LIB_PATH, objs):
-        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

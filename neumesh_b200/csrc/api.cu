@@ -19,7 +19,7 @@ int sm_count() {
   int n = c.load(std::memory_order_relaxed);
   if (n == 0) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;   // H100 SXM
     c.store(n, std::memory_order_relaxed);
   }
   return n;

@@ -134,7 +134,7 @@ static int pack_field(const nmb_field_desc* d, nmb_field* f, cudaStream_t stream
   NMB_CHECK(d->geometry_dim >= FEAT && d->geometry_dim % FEAT == 0 && d->color_dim >= FEAT && d->color_dim % FEAT == 0,
             "fused kernels need vertex code widths that are multiples of 32");
   NMB_CHECK(f->engine != 1 || (d->geometry_dim == FEAT && d->color_dim == FEAT),
-            "the fp32 engine is specialised for 32-d vertex codes (use the tcgen05 engine)");
+            "the fp32 engine is specialised for 32-d vertex codes (use a tensor-core engine)");
   NMB_CHECK(d->D_density >= 1 && d->D_density < MAX_LAYERS && d->D_color >= 1 && d->D_color < MAX_LAYERS,
             "unsupported MLP depth");
   NMB_CHECK(d->multires_d >= 0 && d->multires_fg >= 0 && d->multires_ft >= 0 && d->multires_view >= 0,
@@ -201,7 +201,7 @@ int nmb_field_create(const nmb_grid* g, const nmb_field_desc* desc, int mlp_engi
   if (!out) return 2;
   *out = nullptr;
   NMB_CHECK(g != nullptr && desc != nullptr, "null grid / descriptor");
-  NMB_CHECK(mlp_engine >= 0 && mlp_engine <= 2, "mlp_engine must be 0 (tcgen05 3xTF32), 1 (fp32) or 2 (tcgen05 fp16x3)");
+  NMB_CHECK(mlp_engine >= 0 && mlp_engine <= 2, "mlp_engine must be 0 (tensor-core 3xTF32), 1 (fp32) or 2 (tensor-core fp16x3)");
   nmb_field* f = new nmb_field();
   f->grid = g;
   f->engine = mlp_engine;

@@ -33,7 +33,7 @@ struct MlpFfma {            // fp32 engine: W^T per layer, [K][256] row-major (k
   int n_layers = 0, n_out = 0;
 };
 
-struct MlpTc {              // tcgen05 engine: per layer, per 16-column K-slab: [hi | lo] x [K/4][256][4] tf32 images
+struct MlpTc {              // tensor-core engine: per layer, per 16-column K-slab: [hi | lo] x [K/4][256][4] tf32 images
   DevBuf<float> w;
   DevBuf<int32_t> kmap[MAX_LAYERS];   // packing only: source column of every packed K column (kept between re-packs)
   int64_t slab_off[MAX_LAYERS];  // in floats

@@ -1,31 +1,30 @@
-// tcgen05 MLP engines (mlp_engine = 2: fp16x3 split operands, the default; mlp_engine = 0: 3xTF32): the NeuMesh
-// geometry / colour MLPs on the 5th-generation tensor cores.
+// Tensor-core MLP engines for Hopper (sm_90a; mlp_engine = 2: fp16x3 split operands, the default; mlp_engine = 0:
+// 3xTF32): the NeuMesh geometry / colour MLPs on wgmma.  The Python-side engine names ("tcgen05_f16", "tcgen05") are
+// kept for API compatibility.
 //
 // Why split operands.  The sdf feeds sigmoid(s * sdf) with s ~ 50-300 and a discrete re-sampling cascade; single-pass TF32
 // (10-bit mantissa) or BF16 operands miss the 1e-4 / 1e-5 parity bar by 1-3 orders of magnitude, while the split
-// x = hi + lo (both TF32), D += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi with fp32 accumulation in TMEM is fp32-accurate
+// x = hi + lo (both TF32), D += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi with fp32 accumulation is fp32-accurate
 // (SURVEY.md section 7.3); the fp16 variant (hi = fp16(x), lo = fp16(x - hi), weights pre-scaled by 2^8) is as accurate
-// at twice the MMA rate and half the operand bytes.  Every algorithmic MAC is therefore issued three times: tensor-pipe
-// utilisation is quoted against ISSUED MMAs and the 3x factor is stated wherever a FLOP/s figure appears.
+// at twice the MMA rate and half the operand bytes.  Every algorithmic MAC is therefore issued three times.
 //
-// One persistent CTA per SM (clusters of 2 share every weight slab), 128 rows (points) per tile, warp-specialised:
-//   warps 0-15  epilogue : TMEM -> registers (tcgen05.ld), bias + activation, hi/lo split, next layer's A slabs -> smem;
-//                          quadrant = w & 3 (TMEM lanes), chunk parity = (w >> 2) & 1, column half = w >> 3
-//   warps 16-23 builder  : neighbour gather + blend + positional encoding -> first-layer A slabs (2 threads per row)
-//   warp  24    MMA      : one lane issues tcgen05.mma (M = 128, N = 256; kind::f16 K = 16 or kind::tf32 K = 8) and the
-//                          tcgen05.commit that release ring slots / publish the accumulator
-//   warp  25    loader   : weight slabs L2 -> smem with cp.async.bulk (TMA 1-D bulk copy, cluster multicast) + complete_tx
-// Layer l's 128x256 fp32 accumulator lives in TMEM columns [256*(l&1), +256); while the epilogue drains it 16 columns
-// at a time into K-slabs of layer l+1, the MMA warp is already accumulating layer l+1 into the other half.
-// Schedules that were built and measured slower on B200 (CTA pairs with cta_group::2, two tiles per CTA, shuffle exchange
-// for the tangent rows, packed f32x2 epilogue arithmetic): profiles/r2_mlp_schedule_experiments.txt, DESIGN.md 4.2.
+// One persistent CTA per SM.  Every consumer warpgroup owns a 64-row tile (points; in the geometry + tangent mode rows
+// 32..63 carry d/d(ds) of rows 0..31) and does all the work for it:
+//   * layer 0: its threads build the first-layer A slabs (neighbour gather + blend + positional encoding, 2 threads per
+//     row) into a 2-step ring inside the warpgroup's shared-memory region; the wgmma of step s runs while step s + 1 is
+//     being built;
+//   * every layer: wgmma m64n256 (k16 fp16 / k8 tf32) with the 64x256 fp32 accumulator in registers (128 per thread);
+//   * epilogue: bias + activation, hi/lo split, the whole next-layer A operand (64 rows x 256 K) written back into the
+//     region, or the output layer's dot products (quad shuffles) for the last layer.
+// The fp16 engine runs two consumer warpgroups per CTA (two 64 KB regions), the TF32 engine one (its A operand is
+// 128 KB).  One producer thread streams the weight slabs L2 -> shared memory with cp.async.bulk into a ring that the
+// CTA's warpgroups consume in lock step (mbarrier full / empty pairs).
 //
-// Operand layout (no-swizzle, K-major "interleave" canonical layout): a K-slab of 16 columns is stored as
-// [k/4][row][k%4] fp32, i.e. 8x16-byte core matrices with SBO = 128 B (next 8 rows) and LBO = rows*16 B (next 4 k).
-// Weights are pre-packed in exactly this image (hi slab then lo slab) so a slab is ONE contiguous 32 KB bulk copy.
+// Operand layout (no swizzle, K-major canonical layout): a K-slab of 16 columns is stored as [k/4][row][k%4] fp32 (tf32)
+// or [k/8][row][k%8] fp16, i.e. 8x16-byte core matrices with SBO = 128 B (next 8 rows) and LBO = rows*16 B (next
+// k chunk).  Weights are pre-packed in exactly this image (hi slab then lo slab), so a slab is one contiguous copy.
 #include <cuda_fp16.h>
 
-#include <cstdlib>
 #include <vector>
 
 #include "field_build.cuh"
@@ -34,61 +33,52 @@ namespace nmb {
 
 namespace tc {
 
-constexpr int ROWS = 128;                  // tile rows (TMEM lanes)
-constexpr int SLAB_K = 16;                 // K columns per pipeline slab
-constexpr int A_HALF = ROWS * SLAB_K * 4;  // 8 KB: one hi (or lo) A slab
-constexpr int A_SLOT = 2 * A_HALF;         // 16 KB
-constexpr int B_HALF = MLP_W * SLAB_K * 4; // 16 KB
-constexpr int B_SLOT = 2 * B_HALF;         // 32 KB
-constexpr int NA0 = 2;                     // first-layer A ring (builder -> MMA)
-constexpr int NA1 = 4;                     // hidden-layer A ring (epilogue -> MMA)
-constexpr int NA = NA0 + NA1;
-constexpr int NB = 3;                      // B ring slots (loader -> MMA)
-constexpr int CLUSTER = 2;                 // CTAs per cluster sharing every weight slab through TMA multicast
-// NOTE two separate A rings: an mbarrier parity wait is only meaningful while the waiter is at most one phase
-// ahead of the barrier.  The builder runs a whole tile ahead of the epilogue, so the two producer groups must not
-// share one ring (a shared ring deadlocks as soon as a CTA processes a second tile).
-constexpr int N_EPI = 512;                 // 16 warps: quadrant = w & 3 (TMEM lanes), group g = (w >> 2) & 1 drains the chunks
-                                           // j with j % 2 == g, half hh = w >> 3 takes columns [8 hh, 8 hh + 8) of a chunk
-constexpr int N_BUILD = 256;               // 2 threads per row: half h builds columns [8h, 8h+8) of every first-layer slab
-constexpr int THREADS = N_EPI + N_BUILD + 64;
-constexpr int WARP_BUILD = N_EPI / 32, WARP_MMA = (N_EPI + N_BUILD) / 32;
-constexpr int SIG_BUF = 64 * 16;           // floats per exp(100 z) exchange buffer (64 value rows x 16 columns)
-constexpr int CONST_FLOATS = (MAX_LAYERS + 3) * MLP_W;   // biases of every hidden layer + up to 3 output rows
-
-// fp16x3 operand variant (mlp_engine = 2): the same slabs with fp16 hi / lo images - half the bytes, and a 16-column
-// slab is ONE kind::f16 K step (K = 16) instead of two tf32 ones.  The halved slots buy rings twice as deep.
-constexpr int A_HALF16 = ROWS * SLAB_K * 2;   // 4 KB
-constexpr int A_SLOT16 = 2 * A_HALF16;        // 8 KB
-constexpr int B_HALF16 = MLP_W * SLAB_K * 2;  // 8 KB
+constexpr int ROWS = 64;                      // rows of a warpgroup tile (wgmma M)
+constexpr int SLAB_K = 16;                    // K columns per slab
+constexpr int B_HALF32 = MLP_W * SLAB_K * 4;  // 16 KB: one hi (or lo) tf32 weight slab
+constexpr int B_SLOT32 = 2 * B_HALF32;        // 32 KB
+constexpr int B_HALF16 = MLP_W * SLAB_K * 2;  // 8 KB: one hi (or lo) fp16 weight slab
 constexpr int B_SLOT16 = 2 * B_HALF16;        // 16 KB
 constexpr float F16_W_SCALE = 256.f;          // weights are packed as 2^8 W (keeps their lo parts out of the subnormals)
-// Synchronisation step of the fp16 engine: GR16 = 2 slabs (32 K-columns) share ONE ring slot, i.e. one full / empty
-// barrier pair and one tcgen05.commit pair.  Measured in round 2 (profiles/r2_mlp_schedule_experiments.txt): the single
-// MMA-issuing thread pays ~560 clk of fixed cost per ring step (two barrier polls, tcgen05.fence, descriptors, two
-// commits - one of them cluster-multicast) against ~50 clk per MMA it issues, and that fixed cost - not the tensor core -
-// bounded the engine; one step per 32 columns halves it.  Ring depths below are in steps.
+// fp16 engine: GR16 = 2 slabs (32 K-columns) per pipeline step, i.e. per weight-ring slot and barrier pair; the first
+// layer is padded with zero slabs to whole steps
 constexpr int GR16 = 2;
-constexpr int NA0_16 = 2, NA1_16 = 4, NA_16 = NA0_16 + NA1_16, NB_16 = 3;
+constexpr int NB = 2;                         // weight ring depth (steps)
+constexpr int NA0 = 2;                        // first-layer A ring depth (steps) inside a warpgroup's region
+constexpr int CONST_FLOATS = (MAX_LAYERS + 3) * MLP_W;   // biases of every hidden layer + up to 3 output rows
+constexpr int SIG_FLOATS = 64 * 32;           // per warpgroup: exp(100 z) of one column quarter of the value rows
 
-// SIG: the kernel instantiation exchanges exp(100 z) between value and tangent rows (MODE 1); the others spend those
-// 16 KB on one more first-layer ring step (the MMA thread waits for the builder ~10 % of its time with two)
-template <bool F16, bool SIG = true>
-struct SmemLayoutT {
-  static constexpr int NA0_ = F16 ? (SIG ? NA0_16 : NA0_16 + 1) : NA0;
-  static constexpr int a_off = 0;
-  static constexpr int b_off = F16 ? (NA0_ + NA1_16) * GR16 * A_SLOT16 : NA * A_SLOT;
-  static constexpr int sig_off = b_off + (F16 ? NB_16 * GR16 * B_SLOT16 : NB * B_SLOT);   // [group][parity] buffers
-  static constexpr int part_off = sig_off + ((SIG || !F16) ? 4 * SIG_BUF * 4 : 0);   // last-layer partial sums: [3 helpers][3][128]
-  static constexpr int const_off = part_off + 9 * ROWS * 4;    // biases + output weights
-  static constexpr int bar_off = const_off + CONST_FLOATS * 4;
-  static constexpr int total = bar_off + (F16 ? 512 : 256);   // 2 (NA + NB) + 4 mbarriers + the TMEM base address
+template <bool F16>
+struct Cfg {
+  static constexpr int NWG = F16 ? 2 : 1;                        // consumer warpgroups per CTA
+  static constexpr int GR = F16 ? GR16 : 1;                      // slabs per pipeline step
+  static constexpr int A_HALF = ROWS * SLAB_K * (F16 ? 2 : 4);   // one hi (or lo) A slab
+  static constexpr int A_SUB = 2 * A_HALF;                       // one A slab, hi + lo
+  static constexpr int A_REGION = (MLP_W / SLAB_K) * A_SUB;      // a whole 256-column A operand: 64 KB / 128 KB
+  static constexpr int B_HALF = F16 ? B_HALF16 : B_HALF32;
+  static constexpr int B_SUB = F16 ? B_SLOT16 : B_SLOT32;
+  static constexpr int B_STEP = GR * B_SUB;                      // 32 KB
+  // + the producer: one warp, or with two consumer warpgroups a whole warpgroup so that setmaxnreg can hand its
+  // registers to the consumers (a 288-thread block would cap every thread at 168 registers and spill the accumulator)
+  static constexpr int THREADS = NWG * 128 + (NWG > 1 ? 128 : 32);
+  static constexpr int REGS_CONSUMER = 232, REGS_PRODUCER = 40;  // NWG > 1: 2 * 128 * 232 + 128 * 40 <= 65536
 };
-using SmemLayout = SmemLayoutT<false>;
-static_assert(SmemLayoutT<true, true>::total <= 232448 && SmemLayoutT<true, false>::total <= 232448,
-              "shared memory budget (fp16 variant)");
-static_assert((2 * (NA_16 + 1 + NB_16) + 4) * 8 + 4 <= 512 && (2 * (NA + NB) + 4) * 8 + 4 <= 256, "mbarrier block");
-static_assert(SmemLayout::total <= 232448, "shared memory budget");
+
+// SIG: the geometry + tangent instantiation exchanges exp(100 z) between value and tangent rows
+template <bool F16, bool SIG>
+struct SmemLayoutT {
+  using C = Cfg<F16>;
+  static constexpr int a_off = 0;
+  static constexpr int b_off = C::NWG * C::A_REGION;
+  static constexpr int sig_off = b_off + NB * C::B_STEP;
+  static constexpr int const_off = sig_off + (SIG ? C::NWG * SIG_FLOATS * 4 : 0);
+  static constexpr int bar_off = const_off + CONST_FLOATS * 4;
+  static constexpr int total = bar_off + 2 * NB * 8;
+};
+static_assert(SmemLayoutT<true, true>::total <= 232448 && SmemLayoutT<false, true>::total <= 232448,
+              "shared memory budget (227 KB per block)");
+static_assert(NA0 * Cfg<true>::GR * Cfg<true>::A_SUB <= Cfg<true>::A_REGION &&
+              NA0 * Cfg<false>::GR * Cfg<false>::A_SUB <= Cfg<false>::A_REGION, "first-layer ring fits the region");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -113,8 +103,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// single-thread roles (MMA issuer, loader): back off between polls so the spin does not steal issue slots from the
-// epilogue / builder warps that share the scheduler
+// the producer thread backs off between polls so its spin does not steal issue slots from the consumer warps
 __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity) {
   uint32_t done;
   while (true) {
@@ -130,8 +119,6 @@ __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity)
   }
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
@@ -139,108 +126,74 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
                : "memory");
 }
 
-// Multicast variant: the bytes land at the same CTA-relative offset in every CTA of `mask`, and complete_tx is
-// signalled on the mbarrier at the same offset in each of them.
-__device__ __forceinline__ void bulk_load_mc(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type=0 [61,64))
+// wgmma shared-memory matrix descriptor, no swizzle: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout 0 [62,64)
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
 
-// cute::UMMA::InstrDescriptor for kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = 256
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// kind::f16 (A and B fp16, fp32 accumulate), same shape: a_format = b_format = 0 (F16)
-constexpr uint32_t IDESC_F16 = (1u << 4) | (0u << 7) | (0u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(IDESC_F16), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-// the registers are tied to the wait ("+r") so that no consumer can be scheduled ahead of it
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld8_issue(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait8(uint32_t (&r)[8]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7])
-               :
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accumulator accesses across the asynchronous MMA's issue / wait points
+__device__ __forceinline__ void fence_acc(float (&d)[128]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
+// Accumulator fragment of m64n256: d[4 n8 + 2 hh + jj] = D(row 16 warp + lane / 4 + 8 hh, col 8 n8 + 2 (lane % 4) + jj)
+#define NMB_WG_D \
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, " \
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, " \
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, " \
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, " \
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+
+#define NMB_WG_OPS \
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), \
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), \
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), \
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), \
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), \
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), \
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+
+__device__ __forceinline__ void mma_f16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {" NMB_WG_D "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : NMB_WG_OPS
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void mma_tf32(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {" NMB_WG_D "}, %128, %129, p, 1, 1;\n\t}"
+      : NMB_WG_OPS
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+#undef NMB_WG_D
+#undef NMB_WG_OPS
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -254,25 +207,7 @@ __device__ __forceinline__ float tf32_rna(float x) {
   return __uint_as_float(u);
 }
 
-// write 16 consecutive K-columns of row `r` into an A slot: hi half then lo half, [k/4][row][k%4]
-__device__ __forceinline__ void store_a_row(char* a_slot, int r, const float (&v)[16]) {
-#pragma unroll
-  for (int kc = 0; kc < 4; ++kc) {
-    float4 hi, lo;
-    hi.x = tf32_rna(v[kc * 4 + 0]);
-    hi.y = tf32_rna(v[kc * 4 + 1]);
-    hi.z = tf32_rna(v[kc * 4 + 2]);
-    hi.w = tf32_rna(v[kc * 4 + 3]);
-    lo.x = tf32_rna(v[kc * 4 + 0] - hi.x);
-    lo.y = tf32_rna(v[kc * 4 + 1] - hi.y);
-    lo.z = tf32_rna(v[kc * 4 + 2] - hi.z);
-    lo.w = tf32_rna(v[kc * 4 + 3] - hi.w);
-    *reinterpret_cast<float4*>(a_slot + kc * (ROWS * 16) + r * 16) = hi;
-    *reinterpret_cast<float4*>(a_slot + A_HALF + kc * (ROWS * 16) + r * 16) = lo;
-  }
-}
-
-// write 8 consecutive K-columns [8h, 8h+8) of row `r` (two 4-column chunks) into an A slot
+// write 8 consecutive K-columns [8h, 8h+8) of row `r` (two 4-column chunks) into a tf32 A slab: hi, then lo
 __device__ __forceinline__ void store_a_half(char* a_slot, int r, int h, const float (&v)[8]) {
 #pragma unroll
   for (int c = 0; c < 2; ++c) {
@@ -287,11 +222,11 @@ __device__ __forceinline__ void store_a_half(char* a_slot, int r, int h, const f
     lo.z = tf32_rna(v[c * 4 + 2] - hi.z);
     lo.w = tf32_rna(v[c * 4 + 3] - hi.w);
     *reinterpret_cast<float4*>(a_slot + kc * (ROWS * 16) + r * 16) = hi;
-    *reinterpret_cast<float4*>(a_slot + A_HALF + kc * (ROWS * 16) + r * 16) = lo;
+    *reinterpret_cast<float4*>(a_slot + Cfg<false>::A_HALF + kc * (ROWS * 16) + r * 16) = lo;
   }
 }
 
-// fp16 variant of store_a_half: the 8 columns [8h, 8h+8) of row `r` are ONE 16-byte chunk ([k/8][row][k%8] halves);
+// fp16 variant: the 8 columns [8h, 8h+8) of row `r` are ONE 16-byte chunk ([k/8][row][k%8] halves);
 // hi = fp16(x), lo = fp16(x - hi) (lo may be subnormal: absolute error <= 2^-25, see tools/split_precision_study.py)
 __device__ __forceinline__ void store_a_half_f16(char* a_slot, int r, int h, const float (&v)[8]) {
   uint32_t hi[4], lo[4];
@@ -304,7 +239,28 @@ __device__ __forceinline__ void store_a_half_f16(char* a_slot, int r, int h, con
     lo[c] = *reinterpret_cast<const uint32_t*>(&lp);
   }
   *reinterpret_cast<uint4*>(a_slot + h * (ROWS * 16) + r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-  *reinterpret_cast<uint4*>(a_slot + A_HALF16 + h * (ROWS * 16) + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  *reinterpret_cast<uint4*>(a_slot + Cfg<true>::A_HALF + h * (ROWS * 16) + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
+
+// the two adjacent columns (c, c + 1) of row `r` of a whole-layer A operand (epilogue -> next layer)
+template <bool F16>
+__device__ __forceinline__ void store_a_pair(char* region, int r, int c, float x0, float x1) {
+  using C = Cfg<F16>;
+  char* slab = region + (c >> 4) * C::A_SUB;
+  const int k = c & 15;
+  if constexpr (F16) {
+    const __half2 hp = __floats2half2_rn(x0, x1);
+    const float2 hf = __half22float2(hp);
+    const __half2 lp = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+    char* dst = slab + (k >> 3) * (ROWS * 16) + r * 16 + (k & 7) * 2;
+    *reinterpret_cast<__half2*>(dst) = hp;
+    *reinterpret_cast<__half2*>(dst + C::A_HALF) = lp;
+  } else {
+    const float h0 = tf32_rna(x0), h1 = tf32_rna(x1);
+    char* dst = slab + (k >> 2) * (ROWS * 16) + r * 16 + (k & 3) * 4;
+    *reinterpret_cast<float2*>(dst) = make_float2(h0, h1);
+    *reinterpret_cast<float2*>(dst + C::A_HALF) = make_float2(tf32_rna(x0 - h0), tf32_rna(x1 - h1));
+  }
 }
 
 struct Params {
@@ -318,290 +274,173 @@ struct Params {
   int64_t slab_off[MAX_LAYERS];  // floats
   int n_slabs[MAX_LAYERS];
   int n_layers;
-  int slabs_per_tile;
   int64_t P;
   float* out0;
   float* out1;
-  unsigned long long* dbg;   // optional [8] cycle counters (NMB_TC_PROFILE=1): where the pipeline waits
 };
-
-// wait that accounts its cycles into `acc` when profiling
-__device__ __forceinline__ void mbar_wait_t(uint32_t bar, uint32_t parity, bool prof, unsigned long long& acc) {
-  if (!prof) {
-    mbar_wait(bar, parity);
-    return;
-  }
-  const long long t0 = clock64();
-  mbar_wait(bar, parity);
-  acc += (unsigned long long)(clock64() - t0);
-}
-__device__ __forceinline__ void mbar_wait_bt(uint32_t bar, uint32_t parity, bool prof, unsigned long long& acc) {
-  if (!prof) {
-    mbar_wait_backoff(bar, parity);
-    return;
-  }
-  const long long t0 = clock64();
-  mbar_wait_backoff(bar, parity);
-  acc += (unsigned long long)(clock64() - t0);
-}
 
 }  // namespace tc
 
-// MODE 0: geometry, 128 points / tile.  MODE 1: geometry + tangent rows (rows 64..127 carry d/d(ds) of rows 0..63).
-// MODE 2: colour, 128 points / tile.
-// F16 = false: 3xTF32 operands (mlp_engine 0).  F16 = true: fp16x3 operands (mlp_engine 2, see A_HALF16 above).
+// MODE 0: geometry.  MODE 1: geometry + tangent rows (rows 32..63 of a warpgroup tile carry d/d(ds) of rows 0..31).
+// MODE 2: colour.
+// F16 = false: 3xTF32 operands (mlp_engine 0).  F16 = true: fp16x3 operands (mlp_engine 2).
 template <int MODE, bool F16 = false>
-__global__ void __cluster_dims__(tc::CLUSTER, 1, 1) __launch_bounds__(tc::THREADS, 1)
-mlp_tc_kernel(const tc::Params prm) {
+__global__ void __launch_bounds__(tc::Cfg<F16>::THREADS, 1) mlp_tc_kernel(const tc::Params prm) {
   using namespace tc;
+  using C = Cfg<F16>;
   using SmemLayout = SmemLayoutT<F16, MODE == 1>;
-  constexpr int GR = F16 ? GR16 : 1;   // 16-column slabs per ring slot (synchronisation step)
-  constexpr int A_HALF = F16 ? A_HALF16 : tc::A_HALF, A_SUB = F16 ? A_SLOT16 : tc::A_SLOT, A_SLOT = GR * A_SUB;
-  constexpr int B_HALF = F16 ? B_HALF16 : tc::B_HALF, B_SUB = F16 ? B_SLOT16 : tc::B_SLOT, B_SLOT = GR * B_SUB;
-  constexpr int NA0 = SmemLayout::NA0_, NA1 = F16 ? NA1_16 : tc::NA1, NA = NA0 + NA1, NB = F16 ? NB_16 : tc::NB;
+  constexpr int NWG = C::NWG, GR = C::GR, A_SUB = C::A_SUB, B_SUB = C::B_SUB;
+  constexpr int PTS = (MODE == 1) ? ROWS / 2 : ROWS;   // points per warpgroup tile
   extern __shared__ __align__(1024) char smem[];
-  char* a_ring = smem + SmemLayout::a_off;
-  char* b_ring = smem + SmemLayout::b_off;
-  float* sig = reinterpret_cast<float*>(smem + SmemLayout::sig_off);
-  float* part = reinterpret_cast<float*>(smem + SmemLayout::part_off);
   float* cst = reinterpret_cast<float*>(smem + SmemLayout::const_off);   // [n_layers][256] biases, then output rows
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SmemLayout::bar_off);
-  // A_FULL / A_EMPTY: slots [0, NA0) belong to the first-layer ring, [NA0, NA) to the hidden-layer ring
-  constexpr int A_FULL = 0, A_EMPTY = NA, B_FULL = 2 * NA, B_EMPTY = 2 * NA + NB, D_FULL = 2 * NA + 2 * NB,
-                D_EMPTY = D_FULL + 2, N_BARS = D_EMPTY + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + N_BARS);
+  constexpr int B_FULL = 0, B_EMPTY = NB;
   const uint32_t bar0 = smem_u32(bars);
   auto bar = [&](int i) { return bar0 + 8u * (uint32_t)i; };
+  const uint32_t b_base = smem_u32(smem + SmemLayout::b_off);
 
   const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  constexpr int PTS = (MODE == 1) ? 64 : 128;
-  constexpr int N_CHUNK = MLP_W / SLAB_K;
-  const int64_t n_tiles_real = (prm.P + PTS - 1) / PTS;
-  // every CTA runs the SAME number of tiles (padding with all-invalid tiles): the CTAs of a cluster consume the
-  // weight-slab stream in lock step, so none may stop early
-  const int64_t n_tiles = ((n_tiles_real + gridDim.x - 1) / gridDim.x) * gridDim.x;
+  const int64_t n_tiles = (prm.P + NWG * PTS - 1) / (NWG * PTS);   // a CTA tile = one tile per consumer warpgroup
   const FieldLayout& L = prm.lay;
   const int NL = prm.n_layers;
 
   if (tid == 0) {
-    for (int i = 0; i < NA; ++i) {
-      // two half-row producers per row and slab (builders for slots < NA0, epilogue otherwise)
-      mbar_init(bar(A_FULL + i), 256 * GR);
-      mbar_init(bar(A_EMPTY + i), 1);
-    }
     for (int i = 0; i < NB; ++i) {
       mbar_init(bar(B_FULL + i), 1);
-      mbar_init(bar(B_EMPTY + i), CLUSTER);   // released by the MMA warps of every CTA in the cluster
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar(D_FULL + i), 1);
-      mbar_init(bar(D_EMPTY + i), N_EPI);
+      mbar_init(bar(B_EMPTY + i), 4 * NWG);   // released by lane 0 of every consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   {
     const int n_out = (MODE == 2) ? 3 : 1;
-    for (int i = tid; i < prm.n_layers * MLP_W; i += THREADS) cst[i] = prm.bias[i];
-    for (int i = tid; i < n_out * MLP_W; i += THREADS) cst[prm.n_layers * MLP_W + i] = prm.w_out[i];
+    for (int i = tid; i < prm.n_layers * MLP_W; i += C::THREADS) cst[i] = prm.bias[i];
+    for (int i = tid; i < n_out * MLP_W; i += C::THREADS) cst[prm.n_layers * MLP_W + i] = prm.w_out[i];
   }
-  if (warp == WARP_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();   // barriers of every CTA in the cluster are initialised before any multicast can reach them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  __syncthreads();
 
-  if (warp < WARP_BUILD) {
-    // =========================================== epilogue ===========================================
-    const int grp = (warp >> 2) & 1;           // which half of the chunks this warp drains
-    const int hh = warp >> 3;                  // which 8 columns of a chunk
-    const int r = (warp & 3) * 32 + (tid & 31);            // row == TMEM lane
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    float* sig_g = sig + grp * 2 * SIG_BUF;
-    uint32_t g = 0;                            // global layer counter of this CTA
-    uint32_t it = 0;                           // tile iteration of this CTA
-    const bool prof = prm.dbg != nullptr;
-    unsigned long long t_dfull = 0, t_aempty = 0;
-    const long long t_begin = clock64();
-    constexpr float K_EXP = 144.26950408889634f;       // 100 * log2(e)
-    constexpr float K_LOG = 0.0069314718055994531f;    // ln(2) / 100
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int64_t p = tile * PTS + ((MODE == 1) ? (r & 63) : r);
-      const bool valid = p < prm.P;
-      // hidden-layer ring counter: slabs of layers 1..NL-1 of all tiles of this CTA, in MMA order
-      uint32_t q = it * (uint32_t)(prm.slabs_per_tile - prm.n_slabs[0]);
-      for (int l = 0; l < NL; ++l, ++g) {
-        const uint32_t buf = g & 1u;
-        mbar_wait_t(bar(D_FULL + buf), (g >> 1) & 1u, prof, t_dfull);
-        tc_fence_after();
-        const float* bl = cst + l * MLP_W + 8 * hh;
-        const bool last = (l == NL - 1);
-        float o0 = 0.f, o1 = 0.f, o2 = 0.f;
-        // software-pipelined TMEM reads: the load of this warp's NEXT chunk is in flight while the current one is
-        // being activated / split / stored
-        const uint32_t t_row = tmem_base + lane_base + buf * 256u + (uint32_t)(8 * hh);
-        uint32_t raw[8];
-        tmem_ld8_issue(t_row + (uint32_t)(grp * SLAB_K), raw);
-#pragma unroll 1
-        for (int j = grp; j < N_CHUNK; j += 2) {
-          float v[8];
-          tmem_ld_wait8(raw);
+  if (tid >= NWG * 128) {
+    // =========================================== weight producer ====================================
+    if constexpr (NWG > 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::REGS_PRODUCER));
+    if (tid == NWG * 128) {
+      uint32_t q = 0;
+      for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        for (int l = 0; l < NL; ++l) {
+          const float* src = prm.w + prm.slab_off[l];
+          for (int j = 0; j < prm.n_slabs[l]; j += GR, ++q) {   // GR consecutive slabs are contiguous in the image
+            const uint32_t sb = q % NB;
+            mbar_wait_backoff(bar(B_EMPTY + sb), ((q / NB) & 1u) ^ 1u);
+            mbar_expect_tx(bar(B_FULL + sb), C::B_STEP);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = F16 ? __uint_as_float(raw[i]) * (1.0f / F16_W_SCALE) : __uint_as_float(raw[i]);
-          if (j + 2 < N_CHUNK) tmem_ld8_issue(t_row + (uint32_t)((j + 2) * SLAB_K), raw);
-          if (MODE == 2) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i] + bl[j * 16 + i], 0.f);
-          } else if (MODE == 0) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float z = v[i] + bl[j * 16 + i];
-              const float y = __log2f(1.0f + fast_exp2(z * K_EXP)) * K_LOG;
-              v[i] = z > 0.2f ? z : y;   // 100 z > 20
-            }
-          } else {
-            // MODE 1: value rows (0..63) publish e = exp(100 z); both halves then work in parallel:
-            // value: softplus = log(1 + e) / 100, tangent: sigma'(z) * (W t) with sigma' = e / (1 + e)
-            float* sb = sig_g + ((j >> 1) & 1) * SIG_BUF;
-            float e[8];
-            if (r < 64) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                v[i] = v[i] + bl[j * 16 + i];
-                e[i] = fast_exp2(v[i] * K_EXP);
-              }
-              *reinterpret_cast<float4*>(sb + r * 16 + 8 * hh) = make_float4(e[0], e[1], e[2], e[3]);
-              *reinterpret_cast<float4*>(sb + r * 16 + 8 * hh + 4) = make_float4(e[4], e[5], e[6], e[7]);
-            }
-            if (grp == 0) asm volatile("bar.sync 1, 256;" ::: "memory");
-            else asm volatile("bar.sync 2, 256;" ::: "memory");
-            if (r < 64) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float y = __log2f(1.0f + e[i]) * K_LOG;
-                v[i] = (v[i] > 0.2f) ? v[i] : y;
-              }
-            } else {
-              const float4 e0 = *reinterpret_cast<const float4*>(sb + (r - 64) * 16 + 8 * hh);
-              const float4 e1 = *reinterpret_cast<const float4*>(sb + (r - 64) * 16 + 8 * hh + 4);
-              const float ee[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                // 100 z > 20  <=>  e > exp(20)
-                const float sg = ee[i] > 485165195.4097903f ? 1.f : __fdividef(ee[i], ee[i] + 1.f);
-                v[i] *= sg;
-              }
-            }
+            for (int hf = 0; hf < 2; ++hf)
+              bulk_load(b_base + sb * C::B_STEP + hf * (C::B_STEP / 2), src + (int64_t)j * (B_SUB / 4) + hf * (C::B_STEP / 8),
+                        C::B_STEP / 2, bar(B_FULL + sb));
           }
-          if (!last) {
-            const uint32_t qs = q + (uint32_t)j;          // slab counter; GR consecutive slabs share a ring slot
-            const uint32_t gq = qs / GR;
-            const uint32_t slot = NA0 + gq % NA1;
-            char* a_dst = a_ring + slot * A_SLOT + (qs % GR) * A_SUB;
-            mbar_wait_t(bar(A_EMPTY + slot), ((gq / NA1) & 1u) ^ 1u, prof, t_aempty);
-            if constexpr (F16) store_a_half_f16(a_dst, r, hh, v);
-            else store_a_half(a_dst, r, hh, v);
-            fence_proxy_async();
-            mbar_arrive(bar(A_FULL + slot));
-          } else {
-            const float* wo = cst + NL * MLP_W + j * 16 + 8 * hh;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              o0 = fmaf(v[i], wo[i], o0);
-              if (MODE == 2) {
-                o1 = fmaf(v[i], wo[MLP_W + i], o1);
-                o2 = fmaf(v[i], wo[2 * MLP_W + i], o2);
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(bar(D_EMPTY + buf));
-        if (!last) {
-          q += N_CHUNK;
-        } else {
-          // combine the four partial dot products of a row (helpers -> smem -> warp-group (grp 0, hh 0))
-          const int helper = grp + 2 * hh;   // 0 = finaliser, 1..3 = helpers
-          if (helper != 0) {
-            float* pp = part + (helper - 1) * 3 * ROWS;
-            pp[r] = o0;
-            if (MODE == 2) {
-              pp[ROWS + r] = o1;
-              pp[2 * ROWS + r] = o2;
-            }
-          }
-          asm volatile("bar.sync 3, 512;" ::: "memory");
-          if (helper == 0) {
-#pragma unroll
-            for (int hlp = 0; hlp < 3; ++hlp) {
-              const float* pp = part + hlp * 3 * ROWS;
-              o0 += pp[r];
-              if (MODE == 2) {
-                o1 += pp[ROWS + r];
-                o2 += pp[2 * ROWS + r];
-              }
-            }
-            if (valid) {
-              if (MODE == 2) {
-                prm.out0[0 * prm.in.stride + p] = sigmoid_acc(o0 + __ldg(prm.b_out + 0));
-                prm.out0[1 * prm.in.stride + p] = sigmoid_acc(o1 + __ldg(prm.b_out + 1));
-                prm.out0[2 * prm.in.stride + p] = sigmoid_acc(o2 + __ldg(prm.b_out + 2));
-              } else if (MODE == 0 || r < 64) {
-                prm.out0[p] = o0 + __ldg(prm.b_out);
-              } else if (prm.out1) {
-                const int64_t ps = field_src(prm.in, p);
-                prm.out1[0 * prm.in.stride + p] = o0 * prm.in.grad[0 * prm.in.stride + ps];
-                prm.out1[1 * prm.in.stride + p] = o0 * prm.in.grad[1 * prm.in.stride + ps];
-                prm.out1[2 * prm.in.stride + p] = o0 * prm.in.grad[2 * prm.in.stride + ps];
-              }
-            }
-          }
-          // helpers may only overwrite `part` after the finaliser has read it
-          asm volatile("bar.sync 4, 512;" ::: "memory");
         }
       }
     }
-    if (prof && (tid & 31) == 0) {
-      atomicAdd(prm.dbg + 0, t_dfull);
-      atomicAdd(prm.dbg + 1, t_aempty);
-      atomicAdd(prm.dbg + 2, (unsigned long long)(clock64() - t_begin));
+    return;
+  }
+
+  // ============================================= consumer warpgroup =================================
+  if constexpr (NWG > 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::REGS_CONSUMER));
+  const int wg = tid >> 7, t = tid & 127, warp = t >> 5, lane = t & 31;
+  char* region = smem + SmemLayout::a_off + wg * C::A_REGION;
+  const uint32_t a_base = smem_u32(region);
+  float* sig = reinterpret_cast<float*>(smem + SmemLayout::sig_off) + wg * SIG_FLOATS;
+  const uint32_t wg_bar = 1u + (uint32_t)wg;   // named barrier of this warpgroup (0 is __syncthreads)
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory"); };
+
+  float d[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) d[i] = 0.f;
+  uint32_t qb = 0;    // weight-ring steps consumed by this warpgroup
+  int prev = -1;      // ring slot of the step still in flight (released once its MMAs have completed)
+
+  // one pipeline step: the GR slabs of A at a_addr against the next weight step; returns with at most this step's
+  // MMAs in flight
+  auto step = [&](uint32_t a_addr, bool first) {
+    const uint32_t sb = qb % NB;
+    mbar_wait(bar(B_FULL + sb), (qb / NB) & 1u);
+    const uint32_t b_addr = b_base + sb * C::B_STEP;
+    fence_acc(d);
+    wg_fence();
+#pragma unroll
+    for (int sub = 0; sub < GR; ++sub) {
+      if constexpr (F16) {
+        // one K = 16 step per slab: two 8-column chunks; chunk stride: A 64 rows * 16 B, B 256 rows * 16 B
+        const uint64_t a_hi = make_desc(a_addr + sub * A_SUB, ROWS * 16, 128);
+        const uint64_t a_lo = make_desc(a_addr + sub * A_SUB + C::A_HALF, ROWS * 16, 128);
+        const uint64_t b_hi = make_desc(b_addr + sub * B_SUB, MLP_W * 16, 128);
+        const uint64_t b_lo = make_desc(b_addr + sub * B_SUB + C::B_HALF, MLP_W * 16, 128);
+        mma_f16(d, a_lo, b_hi, (first && sub == 0) ? 0u : 1u);   // small terms first
+        mma_f16(d, a_hi, b_lo, 1u);
+        mma_f16(d, a_hi, b_hi, 1u);
+      } else {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+          // two 4-column chunks per K = 8 step
+          const uint64_t a_hi = make_desc(a_addr + sub * A_SUB + ks * 2 * (ROWS * 16), ROWS * 16, 128);
+          const uint64_t a_lo = make_desc(a_addr + sub * A_SUB + C::A_HALF + ks * 2 * (ROWS * 16), ROWS * 16, 128);
+          const uint64_t b_hi = make_desc(b_addr + sub * B_SUB + ks * 2 * (MLP_W * 16), MLP_W * 16, 128);
+          const uint64_t b_lo = make_desc(b_addr + sub * B_SUB + C::B_HALF + ks * 2 * (MLP_W * 16), MLP_W * 16, 128);
+          mma_tf32(d, a_lo, b_hi, (first && sub == 0 && ks == 0) ? 0u : 1u);
+          mma_tf32(d, a_hi, b_lo, 1u);
+          mma_tf32(d, a_hi, b_hi, 1u);
+        }
+      }
     }
-  } else if (warp < WARP_MMA) {
-    // =========================================== builder ============================================
-    // two threads per row: half h owns features {8g + 4h + i : g < 4, i < 4} and writes columns [8h, 8h+8) of
-    // every first-layer slab (see tc_first_layer_map for the column order)
-    const int tb = tid - N_EPI;
-    const int r = tb & (ROWS - 1);
-    const int h = tb >> 7;
-    uint32_t it = 0;
-    const int off_feat = (MODE == 2) ? L.off_ft : L.off_fg;   // multiple of 16
-    const int Lf = (MODE == 2) ? L.Lft : L.Lfg;
-    const int Fdim = (MODE == 2) ? L.Fc : L.Fg;   // code width = n_fb blocks of FEAT columns
-    const int n_fb = Fdim / FEAT;
-    const float* __restrict__ table = (MODE == 2) ? prm.tab.fc : prm.tab.fg;
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int64_t p = tile * PTS + ((MODE == 1) ? (r & 63) : r);
+    wg_commit();
+    fence_acc(d);
+    wg_wait<1>();   // the previous step's MMAs are complete: its weight slot and A slot may be reused
+    fence_acc(d);
+    if (prev >= 0 && lane == 0) mbar_arrive(bar(B_EMPTY + prev));
+    prev = (int)sb;
+    ++qb;
+  };
+  auto finish_layer = [&]() {
+    wg_wait<0>();
+    fence_acc(d);
+    if (lane == 0) mbar_arrive(bar(B_EMPTY + prev));
+    prev = -1;
+  };
+
+  constexpr float K_EXP = 144.26950408889634f;       // 100 * log2(e)
+  constexpr float K_LOG = 0.0069314718055994531f;    // ln(2) / 100
+  const int off_feat = (MODE == 2) ? L.off_ft : L.off_fg;   // multiple of 16
+  const int Lf = (MODE == 2) ? L.Lft : L.Lfg;
+  const int Fdim = (MODE == 2) ? L.Fc : L.Fg;   // code width = n_fb blocks of FEAT columns
+  const int n_fb = Fdim / FEAT;
+  const float* __restrict__ table = (MODE == 2) ? prm.tab.fc : prm.tab.fg;
+
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int64_t pbase = (tile * NWG + wg) * PTS;
+    // every warp of the warpgroup has seen the previous tile's last MMAs complete before any of them overwrites the
+    // first-layer ring, whose rows the whole warpgroup's MMAs read
+    wg_sync();
+    {
+      // ===================================== layer 0: build + MMA =====================================
+      // two threads per row: half h owns features {8g + 4h + i : g < 4, i < 4} and writes columns [8h, 8h+8) of
+      // every first-layer slab (see tc_first_layer_map for the column order)
+      const int r = t & (ROWS - 1);
+      const int h = t >> 6;
+      const int64_t p = pbase + ((MODE == 1) ? (r & 31) : r);
       const bool valid = p < prm.P;
-      const bool tangent = (MODE == 1) && (r >= 64);
-      uint32_t q = it * (uint32_t)prm.n_slabs[0];   // first-layer ring counter
+      const bool tangent = (MODE == 1) && (r >= 32);
+      uint32_t q = 0;   // first-layer slabs emitted
       auto emit = [&](const float (&v)[8]) {
-        const uint32_t gq = q / GR;                  // q counts slabs; GR consecutive slabs share a ring slot
+        const uint32_t gq = q / GR;                  // GR consecutive slabs share a ring step
         const uint32_t slot = gq % NA0;
-        char* a_dst = a_ring + slot * A_SLOT + (q % GR) * A_SUB;
-        if (q % GR == 0) mbar_wait(bar(A_EMPTY + slot), ((gq / NA0) & 1u) ^ 1u);
+        char* a_dst = region + slot * (GR * A_SUB) + (q % GR) * A_SUB;
         if constexpr (F16) store_a_half_f16(a_dst, r, h, v);
         else store_a_half(a_dst, r, h, v);
-        fence_proxy_async();
-        mbar_arrive(bar(A_FULL + slot));
         ++q;
+        if (q % GR == 0) {
+          fence_proxy_async();
+          wg_sync();
+          step(a_base + slot * (GR * A_SUB), gq == 0);
+        }
       };
-      // ---- gather + blend of this half's 16 features of code block fb (registers).  Block 0 is issued before any
-      //      ring wait so that its latency overlaps the previous tile ----
+      // ---- gather + blend of this half's 16 features of code block fb (registers) ----
       float feat[16];
       float ds = 0.f;
       // where this point's neighbour data lives (geometry modes: optionally indirected, see FieldIn::index)
@@ -686,108 +525,117 @@ mlp_tc_kernel(const tc::Params prm) {
           fr *= 2.f;
         }
       }
-      if constexpr (GR > 1) {   // the first layer is padded with zero slabs (zero weights) to a whole number of ring steps
+      if constexpr (GR > 1) {   // the first layer is padded with zero slabs (zero weights) to a whole number of steps
         const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        while (q < (it + 1u) * (uint32_t)prm.n_slabs[0]) emit(zero);
+        while (q < (uint32_t)prm.n_slabs[0]) emit(zero);
       }
+      finish_layer();
     }
-  } else if (warp == WARP_MMA) {
-    // =========================================== MMA issuer =========================================
-    if ((tid & 31) == 0) {
-      uint32_t g = 0, q = 0, q0 = 0, q1 = 0;   // q: B ring; q0 / q1: first-layer / hidden-layer A rings
-      const uint32_t a0 = smem_u32(a_ring), b0 = smem_u32(b_ring);
-      const bool prof = prm.dbg != nullptr;
-      unsigned long long t_dempty = 0, t_a0 = 0, t_a1 = 0, t_b = 0;
-      const long long t_begin = clock64();
-      for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        for (int l = 0; l < NL; ++l, ++g) {
-          const uint32_t buf = g & 1u;
-          mbar_wait_bt(bar(D_EMPTY + buf), ((g >> 1) & 1u) ^ 1u, prof, t_dempty);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + buf * 256u;
-          const int ns = prm.n_slabs[l];
-          for (int j = 0; j < ns; j += GR, ++q) {   // q, q0, q1 count ring steps of GR slabs
-            uint32_t sa, pa;
-            if (l == 0) {
-              sa = q0 % NA0;
-              pa = (q0 / NA0) & 1u;
-              ++q0;
-            } else {
-              sa = NA0 + q1 % NA1;
-              pa = (q1 / NA1) & 1u;
-              ++q1;
-            }
-            const uint32_t sb = q % NB;
-            mbar_wait_bt(bar(A_FULL + sa), pa, prof, l == 0 ? t_a0 : t_a1);
-            mbar_wait_bt(bar(B_FULL + sb), (q / NB) & 1u, prof, t_b);
-            tc_fence_after();
-            const uint32_t a_addr = a0 + sa * A_SLOT, b_addr = b0 + sb * B_SLOT;
-            if constexpr (F16) {
-#pragma unroll
-              for (int sub = 0; sub < GR; ++sub) {
-                // one K = 16 step per slab: two 8-column chunks; chunk stride: A 128 rows * 16 B, B 256 rows * 16 B
-                const uint64_t a_hi = make_desc(a_addr + sub * A_SUB, ROWS * 16, 128);
-                const uint64_t a_lo = make_desc(a_addr + sub * A_SUB + A_HALF, ROWS * 16, 128);
-                const uint64_t b_hi = make_desc(b_addr + sub * B_SUB, MLP_W * 16, 128);
-                const uint64_t b_lo = make_desc(b_addr + sub * B_SUB + B_HALF, MLP_W * 16, 128);
-                mma_f16(d_tmem, a_lo, b_hi, (j | sub) ? 1u : 0u);   // small terms first
-                mma_f16(d_tmem, a_hi, b_lo, 1u);
-                mma_f16(d_tmem, a_hi, b_hi, 1u);
-              }
-            } else {
-#pragma unroll
-              for (int ks = 0; ks < 2; ++ks) {
-                // two 4-column chunks per K=8 step; chunk stride: A 128 rows * 16 B, B 256 rows * 16 B
-                const uint64_t a_hi = make_desc(a_addr + ks * 2 * (ROWS * 16), ROWS * 16, 128);
-                const uint64_t a_lo = make_desc(a_addr + A_HALF + ks * 2 * (ROWS * 16), ROWS * 16, 128);
-                const uint64_t b_hi = make_desc(b_addr + ks * 2 * (MLP_W * 16), MLP_W * 16, 128);
-                const uint64_t b_lo = make_desc(b_addr + B_HALF + ks * 2 * (MLP_W * 16), MLP_W * 16, 128);
-                mma_tf32(d_tmem, a_lo, b_hi, (j | ks) ? 1u : 0u);   // small terms first
-                mma_tf32(d_tmem, a_hi, b_lo, 1u);
-                mma_tf32(d_tmem, a_hi, b_hi, 1u);
-              }
-            }
-            mma_commit(bar(A_EMPTY + sa));
-            mma_commit_mc(bar(B_EMPTY + sb), (uint16_t)((1u << CLUSTER) - 1u));
-          }
-          mma_commit(bar(D_FULL + buf));
-        }
-      }
-      if (prof) {
-        atomicAdd(prm.dbg + 3, t_dempty);
-        atomicAdd(prm.dbg + 4, t_a0);
-        atomicAdd(prm.dbg + 5, t_a1);
-        atomicAdd(prm.dbg + 6, t_b);
-        atomicAdd(prm.dbg + 7, (unsigned long long)(clock64() - t_begin));
-      }
-    }
-  } else {
-    // =========================================== weight loader ======================================
-    if ((tid & 31) == 0) {
-      uint32_t q = 0;
-      const uint32_t b0 = smem_u32(b_ring);
-      const uint32_t crank = cluster_ctarank();
-      for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        for (int l = 0; l < NL; ++l) {
-          const float* src = prm.w + prm.slab_off[l];
-          for (int j = 0; j < prm.n_slabs[l]; j += GR, ++q) {   // GR consecutive slabs are contiguous in the image
-            const uint32_t sb = q % NB;
-            mbar_wait_backoff(bar(B_EMPTY + sb), ((q / NB) & 1u) ^ 1u);
-            mbar_expect_tx(bar(B_FULL + sb), B_SLOT);
-            // this CTA fetches 1/CLUSTER of the slab from L2 and multicasts it to every CTA of the cluster
-            constexpr uint32_t PART = B_SLOT / CLUSTER;
-            bulk_load_mc(b0 + sb * B_SLOT + crank * PART, src + (int64_t)j * (B_SUB / 4) + crank * (PART / 4), PART,
-                         bar(B_FULL + sb), (uint16_t)((1u << CLUSTER) - 1u));
-          }
-        }
-      }
-    }
-  }
 
-  tc_fence_before();
-  cluster_sync_all();   // no CTA leaves while a peer may still multicast into its shared memory / barriers
-  if (warp == WARP_MMA) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+    // ========================================== layers, epilogues ==========================================
+    const int cq = 2 * (lane & 3);              // first of this thread's two adjacent columns in every 8-column group
+    const int rr = 16 * warp + (lane >> 2);     // this thread's rows: rr and rr + 8
+    for (int l = 0; l < NL; ++l) {
+      if (l > 0) {
+        const int steps = prm.n_slabs[l] / GR;
+        for (int j = 0; j < steps; ++j) step(a_base + j * (GR * A_SUB), j == 0);
+        finish_layer();
+      }
+      const bool last = (l == NL - 1);
+      const float* bl = cst + l * MLP_W;
+      const float* wo = cst + NL * MLP_W;
+      float o[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+      for (int qq = 0; qq < 4; ++qq) {   // column quarters: MODE 1 exchanges exp(100 z) one quarter at a time
+        float v[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = F16 ? d[32 * qq + i] * (1.0f / F16_W_SCALE) : d[32 * qq + i];
+        if (MODE == 2) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i] + bl[8 * (8 * qq + (i >> 2)) + cq + (i & 1)], 0.f);
+        } else if (MODE == 0) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const float z = v[i] + bl[8 * (8 * qq + (i >> 2)) + cq + (i & 1)];
+            const float y = __log2f(1.0f + fast_exp2(z * K_EXP)) * K_LOG;
+            v[i] = z > 0.2f ? z : y;   // 100 z > 20
+          }
+        } else {
+          // MODE 1: value rows (warps 0, 1) publish e = exp(100 z); softplus = log(1 + e) / 100 for the value rows,
+          // sigma'(z) * (W t) with sigma' = e / (1 + e) for the tangent rows (warps 2, 3: same fragment, same point)
+          if (t < 64) {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+              const float z = v[i] + bl[8 * (8 * qq + (i >> 2)) + cq + (i & 1)];
+              const float e = fast_exp2(z * K_EXP);
+              sig[i * 64 + t] = e;
+              v[i] = z > 0.2f ? z : __log2f(1.0f + e) * K_LOG;
+            }
+          }
+          wg_sync();
+          if (t >= 64) {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+              const float e = sig[i * 64 + (t - 64)];
+              // 100 z > 20  <=>  e > exp(20)
+              v[i] *= e > 485165195.4097903f ? 1.f : __fdividef(e, e + 1.f);
+            }
+          }
+          wg_sync();   // the buffer is rewritten by the next quarter
+        }
+        if (!last) {
+#pragma unroll
+          for (int i = 0; i < 32; i += 2) {
+            const int col = 8 * (8 * qq + (i >> 2)) + cq;
+            store_a_pair<F16>(region, rr + 8 * ((i >> 1) & 1), col, v[i], v[i + 1]);
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int col = 8 * (8 * qq + (i >> 2)) + cq + (i & 1);
+            const int hh = (i >> 1) & 1;
+            o[hh][0] = fmaf(v[i], wo[col], o[hh][0]);
+            if (MODE == 2) {
+              o[hh][1] = fmaf(v[i], wo[MLP_W + col], o[hh][1]);
+              o[hh][2] = fmaf(v[i], wo[2 * MLP_W + col], o[hh][2]);
+            }
+          }
+        }
+      }
+      if (!last) {
+        fence_proxy_async();
+        wg_sync();   // the next layer's A operand is complete
+      } else {
+        // the four threads of a quad hold the partial dot products of the same two rows
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            o[hh][k] += __shfl_xor_sync(0xffffffffu, o[hh][k], 1);
+            o[hh][k] += __shfl_xor_sync(0xffffffffu, o[hh][k], 2);
+          }
+        if ((lane & 3) == 0) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int row = rr + 8 * hh;
+            const int64_t p = pbase + ((MODE == 1) ? (row & 31) : row);
+            if (p >= prm.P) continue;
+            if (MODE == 2) {
+              prm.out0[0 * prm.in.stride + p] = sigmoid_acc(o[hh][0] + __ldg(prm.b_out + 0));
+              prm.out0[1 * prm.in.stride + p] = sigmoid_acc(o[hh][1] + __ldg(prm.b_out + 1));
+              prm.out0[2 * prm.in.stride + p] = sigmoid_acc(o[hh][2] + __ldg(prm.b_out + 2));
+            } else if (MODE == 0 || row < 32) {
+              prm.out0[p] = o[hh][0] + __ldg(prm.b_out);
+            } else if (prm.out1) {
+              const int64_t ps = field_src(prm.in, p);
+              prm.out1[0 * prm.in.stride + p] = o[hh][0] * prm.in.grad[0 * prm.in.stride + ps];
+              prm.out1[1 * prm.in.stride + p] = o[hh][0] * prm.in.grad[1 * prm.in.stride + ps];
+              prm.out1[2 * prm.in.stride + p] = o[hh][0] * prm.in.grad[2 * prm.in.stride + ps];
+            }
+          }
+        }
+      }
+    }
   }
 }
 
@@ -806,10 +654,10 @@ __global__ void pack_tc_kernel(const float* __restrict__ wt /*[K_src][256]*/, co
   const float hi = tc::tf32_rna(x);
   const float lo = tc::tf32_rna(x - hi);
   const int slab = k / tc::SLAB_K, kk = k % tc::SLAB_K;
-  float* base = dst + (int64_t)slab * (tc::B_SLOT / 4);
+  float* base = dst + (int64_t)slab * (tc::B_SLOT32 / 4);
   const int off = (kk / 4) * (MLP_W * 4) + n * 4 + (kk % 4);
   base[off] = hi;
-  base[tc::B_HALF / 4 + off] = lo;
+  base[tc::B_HALF32 / 4 + off] = lo;
 }
 
 // fp16x3 variant: per slab [hi | lo] x [k/8][256][k%8] halves of 2^8 W (hi = fp16(x), lo = fp16(x - hi))
@@ -860,7 +708,7 @@ static std::vector<int32_t> tc_first_layer_map(const FieldLayout& L, bool color)
 static int pack_one(const MlpFfma& src, const FieldLayout& L, bool color, bool f16, MlpTc* dst, cudaStream_t stream) {
   int64_t total = 0;
   dst->total_slabs = 0;
-  const int slot_floats = (f16 ? tc::B_SLOT16 : tc::B_SLOT) / 4;
+  const int slot_floats = (f16 ? tc::B_SLOT16 : tc::B_SLOT32) / 4;
   for (int l = 0; l < src.n_layers; ++l) {
     dst->n_slabs[l] = src.K[l] / tc::SLAB_K;
     if (f16) dst->n_slabs[l] = (int)align_up((int64_t)dst->n_slabs[l], (int64_t)tc::GR16);   // whole ring steps (zero slabs)
@@ -915,50 +763,26 @@ static int launch_tc(const nmb_field* f, const MlpFfma& fm, const MlpTc& tm, con
   prm.bias = fm.b.p;
   prm.w_out = fm.w_out.p;
   prm.b_out = fm.b_out.p;
-  prm.slabs_per_tile = 0;
   for (int i = 0; i < MAX_LAYERS; ++i) {
     prm.slab_off[i] = tm.slab_off[i];
     prm.n_slabs[i] = i < fm.n_layers ? tm.n_slabs[i] : 0;
-    prm.slabs_per_tile += prm.n_slabs[i];
   }
   prm.n_layers = fm.n_layers;
   prm.P = P;
   prm.out0 = out0;
   prm.out1 = out1;
-  prm.dbg = nullptr;
-  static const bool want_prof = getenv("NMB_TC_PROFILE") != nullptr;
-  unsigned long long* dbg_dev = nullptr;   // diagnostics only: allocated per launch, the launch is synchronous then
-  if (want_prof) {
-    NMB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&dbg_dev), 8 * sizeof(unsigned long long)));
-    NMB_CUDA_OK(cudaMemsetAsync(dbg_dev, 0, 8 * sizeof(unsigned long long), stream));
-    prm.dbg = dbg_dev;
-  }
-  constexpr int PTS = (MODE == 1) ? 64 : 128;
+  using C = tc::Cfg<F16>;
+  constexpr int PTS = (MODE == 1) ? tc::ROWS / 2 : tc::ROWS;
   const size_t smem = tc::SmemLayoutT<F16, MODE == 1>::total;
   static DeviceOnce attr_once;
   NMB_CUDA_OK(attr_once.run([&] {
     return cudaFuncSetAttribute(mlp_tc_kernel<MODE, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }));
-  const int64_t tiles = ceil_div(P, PTS);
-  int64_t grid = tiles < (int64_t)sm_count() ? tiles : (int64_t)sm_count();
-  grid = align_up(grid, tc::CLUSTER);
-  if (grid > sm_count()) grid -= tc::CLUSTER;
-  if (grid < tc::CLUSTER) grid = tc::CLUSTER;
+  const int64_t tiles = ceil_div(P, (int64_t)C::NWG * PTS);
+  const int64_t grid = tiles < (int64_t)sm_count() ? tiles : (int64_t)sm_count();
   ProfScope prof(MODE == 2 ? PROF_COLOR : (MODE == 1 ? PROF_GEO_JVP : PROF_GEO), P, stream);
-  mlp_tc_kernel<MODE, F16><<<(unsigned)grid, tc::THREADS, smem, stream>>>(prm);
+  mlp_tc_kernel<MODE, F16><<<(unsigned)grid, C::THREADS, smem, stream>>>(prm);
   NMB_LAUNCH_OK();
-  if (want_prof) {
-    unsigned long long h[8];
-    NMB_CUDA_OK(cudaMemcpyAsync(h, dbg_dev, sizeof(h), cudaMemcpyDeviceToHost, stream));
-    NMB_CUDA_OK(cudaStreamSynchronize(stream));
-    const double ne = 16.0 * grid, nm = 1.0 * grid;  // 16 epilogue warps and 1 MMA thread per CTA report
-    fprintf(stderr,
-            "[tc-prof] mode %d P %lld grid %lld | epilogue warp avg cycles: total %.0f wait D_FULL %.0f wait A_EMPTY %.0f | "
-            "MMA thread: total %.0f wait D_EMPTY %.0f wait A_FULL(L0) %.0f wait A_FULL(hidden) %.0f wait B_FULL %.0f\n",
-            MODE, (long long)P, (long long)grid, h[2] / ne, h[0] / ne, h[1] / ne, h[7] / nm, h[3] / nm, h[4] / nm,
-            h[5] / nm, h[6] / nm);
-    cudaFree(dbg_dev);
-  }
   return 0;
 }
 

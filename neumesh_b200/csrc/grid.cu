@@ -5,7 +5,7 @@
 //   models/mesh_grid.py:109-119 K=8 query  (r = 100 never binds => exact KNN, squared distances ascending)
 //   models/mesh_grid.py:121-144 inverse-distance weights + indicator-blended signed distance
 //
-// B200-first design.  FRNN's uniform grid degenerates to one cell at r=100 (cell = r/2) and brute-forces all V
+// Design.  FRNN's uniform grid degenerates to one cell at r=100 (cell = r/2) and brute-forces all V
 // vertices per query.  Here the vertices are Morton-sorted once and indexed by a sparse octree whose nodes carry
 // TIGHT boxes; a query walks it depth-first, nearest child first, pruning against its current 8th-best distance.
 // That is exact for any query position (the renderer probes the whole unit-sphere chord, far from the surface),
@@ -26,9 +26,9 @@
 
 namespace nmb {
 
-// The directory start of the thread-per-query walk is compiled in only with -DNMB_KNN_DIRECTORY=1: measured on B200 it
-// is bit-identical and not faster (profiles/r2_knn_directory_ab.txt), and merely carrying its code costs the bound scan
-// 12 % (66 -> 75 registers per thread: 59.5 -> 67.6 ms per frame), so the shipped build leaves it out.
+// The directory start of the thread-per-query walk is compiled in only with -DNMB_KNN_DIRECTORY=1: it is bit-identical
+// and was not faster when measured, and merely carrying its code raises the bound scan's register count (66 -> 75 per
+// thread), so the shipped build leaves it out.
 #ifndef NMB_KNN_DIRECTORY
 #define NMB_KNN_DIRECTORY 0
 #endif
@@ -403,8 +403,8 @@ static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb
     NMB_LAUNCH_OK();
   }
   // directory tables: levels [3, min(L - 1, 7)] (finer cells than the vertex spacing buy nothing).  OPT-IN
-  // (build with -DNMB_KNN_DIRECTORY=1 and set NMB_KNN_DIR=1; the cooperative kernels, NMB_KNN_COOP=1, use it too): measured on B200 the directory start is bit-identical but not faster (knn 130.2 -> 133.7 ms, live
-  // lists 43.4 -> 48.3 ms per 800x800 frame, profiles/r2_knn_directory_ab.txt): with a warm bound the ball meets only 1-2
+  // (build with -DNMB_KNN_DIRECTORY=1 and set NMB_KNN_DIR=1; the cooperative kernels, NMB_KNN_COOP=1, use it too): the
+  // directory start is bit-identical but was not faster when measured: with a warm bound the ball meets only 1-2
   // children per TOP level, so the levels it skips cost about as much as the 2x2x2-cell seeding does; the expansions that
   // dominate a walk sit at the bottom levels, where cells are as small as the ball.
   g->dir_lmin = 3;
@@ -631,9 +631,9 @@ knn_lists_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pt
 // ------------------------------------------------------------------------------------------------------------
 static bool knn_legacy() {
   // Default: thread-per-query kernels (with the directory start).  NMB_KNN_COOP=1 selects the 8-lanes-per-query
-  // cooperative kernels instead: bit-identical results, measured 2.4x SLOWER on B200 (profiles/r2_ncu_knn_coop_summary.csv:
-  // 2.15x the warp instructions per query - shuffles, ranking, serial insertions - at 16 of 32 active lanes and 29
-  // resident warps), kept as the record of that experiment and as an independent implementation for cross-checks.
+  // cooperative kernels instead: bit-identical results, but they issue about twice the warp instructions per query
+  // (shuffles, ranking, serial insertions) and were measured slower; kept as an independent implementation for
+  // cross-checks.
   static const bool v = getenv("NMB_KNN_COOP") == nullptr;
   return v;
 }

@@ -182,10 +182,10 @@ __device__ __forceinline__ int dir_seed(const GridView& gv, float qx, float qy, 
   return sp;
 }
 
-// ORDER = 0: surviving children are pushed fully sorted (farthest first); ORDER = 1 (default since round 2): only the
+// ORDER = 0: surviving children are pushed fully sorted (farthest first); ORDER = 1 (default): only the
 // NEAREST survivor is put on top of the stack, the others keep child order (7 compare / selects instead of the
 // 19-comparator network; any push order is exact - the pop test prunes - only the pruning efficiency can differ).
-// Measured on B200 (bit-identical results, tools/knn_ab.py): knn 132.9 -> 127.7 ms per 800x800 frame.
+// Both orders give bit-identical results (tools/knn_ab.py compares them).
 template <int K, bool WARM, int ORDER = 1>
 __device__ __forceinline__ void knn_walk(const float4* __restrict__ nodes, const float4* __restrict__ pts, float qx,
                                          float qy, float qz, float (&d)[K], int32_t (&ix)[K],

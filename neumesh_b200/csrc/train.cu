@@ -19,7 +19,7 @@
 //
 // fp32 CUDA-core arithmetic (FFMA): a training step evaluates ~1.3e5 points (512 rays x 255 samples), ~0.5 TFLOP
 // including the backward - milliseconds - and gradients want fp32 accumulation order stability more than tensor-core
-// throughput; the rendering path (field_tc.cu) is where the tcgen05 engine matters.
+// throughput; the rendering path (field_tc.cu) is where the tensor-core engine matters.
 #include <math_constants.h>
 
 #include "../../include/neumesh_b200.h"

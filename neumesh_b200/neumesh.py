@@ -56,9 +56,9 @@ def _mlp_stack(make_linear, act, in_dim, width, depth):
     return nn.Sequential(*mods)
 
 
-# MLP engines of the CUDA library (nmb_field_create's mlp_engine).  "tcgen05_f16" = fp16x3 split operands on
-# tcgen05 kind::f16 (default since round 2: validated on B200 against the oracle, the float64 truth and the reference's
-# frame goldens; 1.3x faster than "tcgen05" = 3xTF32); "fp32" = CUDA-core verification engine.
+# MLP engines of the CUDA library (nmb_field_create's mlp_engine).  "tcgen05_f16" = fp16x3 split operands on fp16 wgmma
+# (default: held to the oracle, the float64 truth and the reference's frame goldens by the tests); "tcgen05" = 3xTF32 on
+# tf32 wgmma; "fp32" = CUDA-core verification engine.  The names predate the Hopper port and are kept for compatibility.
 MLP_ENGINES = {"tcgen05": 0, "fp32": 1, "tcgen05_f16": 2}
 DEFAULT_MLP_ENGINE = "tcgen05_f16"
 

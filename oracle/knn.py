@@ -2,7 +2,7 @@
 
 The reference's only native dependency on the hot path is the third-party package ``frnn``
 (github.com/lxxue/FRNN; version unpinned - ``README.md:25`` gives a URL only; absent from ``environment.yml`` and
-from ``/root/reference``).  Its algorithm (published): counting-sort the points into a uniform grid of cell size
+from the reference repository).  Its algorithm (published): counting-sort the points into a uniform grid of cell size
 ``r / radius_cell_ratio``, then, per query, scan the 3x3x3 neighbouring cells keeping the K closest points that lie
 within ``r`` in a register min-K; results are squared Euclidean distances, optionally sorted ascending, padded with
 -1 when fewer than K points lie within ``r``.

@@ -1,4 +1,4 @@
-"""Frame-scale golden renders of the UNMODIFIED reference (``/root/reference`` imported verbatim on CPU through
+"""Frame-scale golden renders of the UNMODIFIED reference (the checkout named by ``NEUMESH_REFERENCE_ROOT`` imported verbatim on CPU through
 ``ref_harness``) for BASELINE.json configs 1 / 3 / 5, together with the reference's OWN noise floor.
 
 For each config a strided subset of the rays of a real 800 x 800 spiral frame is rendered twice by the reference
@@ -13,7 +13,7 @@ renderer (``models/renderer.py::volume_render``) over the reference ``NeuMesh``:
 (rays outside 1e-4 RGB / 1e-5 depth of ``clean``) does not exceed the reference's self-noise outlier rate
 (``noisy`` vs ``clean``) by more than 3 binomial sigmas.
 
-Run in the build container only (minutes of CPU):  ``python tests/golden/make_frame_golden.py [config1|config3|config5]``.
+Run with the reference checkout present (minutes of CPU):  ``NEUMESH_REFERENCE_ROOT=... python tests/golden/make_frame_golden.py [config1|config3|config5]``.
 """
 from __future__ import annotations
 

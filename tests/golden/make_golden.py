@@ -1,6 +1,6 @@
-"""Generate ``tests/golden/*.npz`` by running the UNMODIFIED reference (``/root/reference``) on CPU.
+"""Generate ``tests/golden/*.npz`` by running the UNMODIFIED reference on CPU.
 
-Run in the build container only:  ``python tests/golden/make_golden.py``.
+``NEUMESH_REFERENCE_ROOT=<reference checkout> python tests/golden/make_golden.py [oracle_pin | train | texture | ...]``.
 The reference holds no golden vectors of its own (SURVEY.md section 4); these files are outputs of the reference's
 Python for the hot path (``models/renderer.py``, ``models/frameworks/neumesh/neumesh.py``, ``models/mesh_grid.py``) with
 the one absent native dependency (``frnn``) replaced by the exact-KNN restatement in ``oracle/knn.py``.
@@ -195,7 +195,80 @@ def make_raycast_case(name, seed):
     print("wrote", path, os.path.getsize(path), "bytes; rays hitting the surface:", int(mask.sum()), "of", mask.numel())
 
 
+def make_oracle_pin_case(name):
+    """What ``tests/test_oracle.py`` pins the oracle and the drop-in renderer against: point outputs, renders (plain,
+    perturbed with injected uniforms) and ``sample_pdf`` of the UNMODIFIED reference on one small case."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import helpers
+    ns = ref_harness.load()
+    cfg = synth.ModelConfig()
+    mesh = synth.icosphere_mesh(3, seed=5)
+    sd = synth.make_state_dict(mesh, cfg, seed=6)
+    ref = ref_harness.build_reference_model(mesh, cfg, sd)
+    out = dict(level=np.int64(3), seed=np.int64(5), state_digest=np.array(state_digest(sd)))
+    # point outputs at helpers.sample_points(500, seed=1)
+    x, v = helpers.sample_points(500, seed=1)
+    with torch.no_grad():
+        out["pts_density_only"] = ref.forward_density_only(x).numpy()
+    s_r, n_r = ref.forward_with_nablas(x.clone())
+    out["pts_sdf_with_nabla"], out["pts_nabla"] = s_r.detach().numpy(), n_r.detach().numpy()
+    out["pts_rgb"] = ref.forward(x.clone(), v)[1].detach().numpy()
+    # 10 x 10 render, detailed outputs
+    o, d = synth.frame_rays(10, 10, view=1)
+    with torch.no_grad():
+        _, _, ex = ns.renderer.volume_render(o, d, ref, detailed_output=True, rayschunk=64, calc_normal=True,
+                                             white_bkgd=True, bounded_near_far=True)
+    for k in ("rgb", "depth_volume", "mask_volume", "normals_volume", "d_final", "implicit_surface", "radiance"):
+        out["render_" + k] = ex[k].numpy()
+    # sample_pdf on its own, incl. the u = 0 / u = 1 ends
+    torch.manual_seed(0)
+    bins = torch.sort(torch.rand(64, 40), dim=-1)[0]
+    wts = torch.rand(64, 39) * (torch.rand(64, 39) > 0.5)
+    out["pdf_bins"], out["pdf_weights"] = bins.numpy(), wts.numpy()
+    out["pdf_samples"] = ns.rend_util.sample_pdf(bins, wts, 16, det=True).numpy()
+    # 8 x 8 render: output keys and values of a detailed render, keys of a training-style call
+    o, d = synth.frame_rays(8, 8, view=2)
+    kw = dict(calc_normal=True, white_bkgd=True, bounded_near_far=True, detailed_output=True, rayschunk=64)
+    with torch.no_grad():
+        rgb, dep, ex = ns.renderer.volume_render(o, d, ref, **kw)
+    out["small_rgb"], out["small_depth"], out["small_keys"] = rgb.numpy(), dep.numpy(), np.array(sorted(ex.keys()))
+    ref.train()
+    torch.manual_seed(3)
+    _, _, ex_t = ns.renderer.volume_render(o, d, ref, calc_normal=True, detailed_output=True, samples_output=True,
+                                           perturb=True, rayschunk=64)
+    out["train_keys"] = np.array(sorted(ex_t.keys()))
+    ref.eval()
+    # perturb=True with torch.rand patched to hand out these draws (one per up-sampling iteration)
+    o, d = synth.frame_rays(9, 9, view=4)
+    u = torch.rand(4, o.shape[0], 16, generator=torch.Generator().manual_seed(11))
+    calls = {"n": 0}
+    real_rand = torch.rand
+
+    def fake_rand(*shape, **kw):
+        shp = tuple(shape[0]) if len(shape) == 1 and isinstance(shape[0], (list, tuple)) else tuple(shape)
+        r = u[calls["n"]].reshape(shp).clone()
+        calls["n"] += 1
+        return r
+
+    torch.rand = fake_rand
+    try:
+        with torch.no_grad():
+            rgb, dep, ex = ns.renderer.volume_render(o, d, ref, detailed_output=True, perturb=True, rayschunk=4096,
+                                                     calc_normal=True, white_bkgd=False, bounded_near_far=True)
+    finally:
+        torch.rand = real_rand
+    assert calls["n"] == 4
+    out["perturb_u"], out["perturb_rgb"], out["perturb_depth"] = u.numpy(), rgb.numpy(), dep.numpy()
+    out["perturb_d_final"] = ex["d_final"].numpy()
+    path = os.path.join(HERE, name + ".npz")
+    np.savez_compressed(path, **out)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "oracle_pin":
+        make_oracle_pin_case("oracle_pin_small")
+        return
     if len(sys.argv) > 1 and sys.argv[1] == "raycast":
         make_raycast_case("ray_casting_small", seed=60)
         return

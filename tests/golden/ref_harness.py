@@ -1,7 +1,6 @@
-"""Import the UNMODIFIED reference (``/root/reference``) on CPU, for golden-vector generation and oracle pinning.
-
-Only usable in the build container (the GPU box has no ``/root/reference``): nothing under ``tests/`` that is
-marked ``gpu``, nor ``bench.py`` / ``smoke()``, imports this module.
+"""Import the UNMODIFIED reference (a checkout of zju3dv/NeuMesh named by ``NEUMESH_REFERENCE_ROOT``) on CPU, for
+golden-vector generation.  No test, ``bench.py`` or ``smoke()`` imports this module: the tests compare against the
+vectors it produced.
 
 * plumbing dependencies that are absent here and irrelevant to the hot path (``addict``, ``imageio``,
   ``skimage``, ``kornia``, ``open3d``) are stubbed in ``sys.modules`` (SURVEY.md section 8c);
@@ -15,7 +14,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("NEUMESH_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("NEUMESH_REFERENCE_ROOT", "")
 REPO_ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
@@ -60,7 +59,7 @@ def load():
         o3d.io = types.SimpleNamespace(read_triangle_mesh=None)
     _stub("frnn", frnn_grid_points=oracle_knn.frnn_grid_points)
 
-    # the reference uses top-level package names (models, utils, dataio): make them resolve to /root/reference
+    # the reference uses top-level package names (models, utils, dataio): make them resolve to REF_ROOT
     # without shadowing this repo's own packages (none of which use those names).
     sys.path.insert(0, REF_ROOT)
     try:

@@ -1,4 +1,4 @@
-"""Throughput of nmb_tr_gemm (hand-written SGEMM of the training path) vs torch.matmul (cuBLAS fp32), B200."""
+"""Throughput of nmb_tr_gemm (hand-written SGEMM of the training path) vs torch.matmul (cuBLAS fp32)."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import torch
