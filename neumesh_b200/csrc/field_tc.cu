@@ -8,8 +8,8 @@
 // (SURVEY.md section 7.3); the fp16 variant (hi = fp16(x), lo = fp16(x - hi), weights pre-scaled by 2^8) is as accurate
 // at twice the MMA rate and half the operand bytes.  Every algorithmic MAC is therefore issued three times.
 //
-// One persistent CTA per SM.  Every consumer warpgroup owns a 64-row tile (points; in the geometry + tangent mode rows
-// 32..63 carry d/d(ds) of rows 0..31) and does all the work for it:
+// One persistent CTA per SM.  Every consumer warpgroup owns a 64-row tile (points, or their tangent rows d/d(ds) in the
+// geometry + tangent mode, see below) and does all the work for it:
 //   * layer 0: its threads build the first-layer A slabs (neighbour gather + blend + positional encoding, 2 threads per
 //     row) into a 2-step ring inside the warpgroup's shared-memory region; the wgmma of step s runs while step s + 1 is
 //     being built;
@@ -20,11 +20,20 @@
 // 128 KB).  One producer thread streams the weight slabs L2 -> shared memory with cp.async.bulk into a ring that the
 // CTA's warpgroups consume in lock step (mbarrier full / empty pairs).
 //
+// Geometry + tangent mode (MODE 1).  fp16 engine: warpgroup 0 holds the 64 value rows of a CTA tile, warpgroup 1 the 64
+// tangent rows of the same points in the same order, so accumulator fragment i of thread t is the same (point, column)
+// in both.  A tangent row's first-layer input is zero outside the head block, so warpgroup 1 builds and multiplies only
+// the ring steps holding head columns and just releases the others.  In each epilogue warpgroup 0 hands e = exp(100 z)
+// to warpgroup 1 one column eighth at a time through two shared-memory buffers (named-barrier full / empty pairs), so
+// the value and tangent formulas run on all four SM sub-partitions and pipeline across eighths.  TF32 engine (one
+// consumer warpgroup): rows 32..63 of a tile carry d/d(ds) of rows 0..31, exchanged one column quarter at a time.
+//
 // Operand layout (no swizzle, K-major canonical layout): a K-slab of 16 columns is stored as [k/4][row][k%4] fp32 (tf32)
 // or [k/8][row][k%8] fp16, i.e. 8x16-byte core matrices with SBO = 128 B (next 8 rows) and LBO = rows*16 B (next
 // k chunk).  Weights are pre-packed in exactly this image (hi slab then lo slab), so a slab is one contiguous copy.
 #include <cuda_fp16.h>
 
+#include <type_traits>
 #include <vector>
 
 #include "field_build.cuh"
@@ -46,7 +55,12 @@ constexpr int GR16 = 2;
 constexpr int NB = 2;                         // weight ring depth (steps)
 constexpr int NA0 = 2;                        // first-layer A ring depth (steps) inside a warpgroup's region
 constexpr int CONST_FLOATS = (MAX_LAYERS + 3) * MLP_W;   // biases of every hidden layer + up to 3 output rows
-constexpr int SIG_FLOATS = 64 * 32;           // per warpgroup: exp(100 z) of one column quarter of the value rows
+// MODE 1 exchange area per consumer warpgroup: exp(100 z) of one column quarter of 32 value rows (TF32 engine), or one
+// of the fp16 engine's two column-eighth buffers ([16 values][128 threads])
+constexpr int SIG_FLOATS = 64 * 32;
+static_assert(SIG_FLOATS == 16 * 128, "an fp16 exchange buffer holds one column eighth of a warpgroup's accumulator");
+// fp16 MODE 1 exchange: named barriers (0 is __syncthreads, 1..2 the consumer warpgroups') of buffers 0 / 1
+constexpr uint32_t EX_FULL = 3, EX_EMPTY = 5;
 
 template <bool F16>
 struct Cfg {
@@ -63,6 +77,13 @@ struct Cfg {
   static constexpr int THREADS = NWG * 128 + (NWG > 1 ? 128 : 32);
   static constexpr int REGS_CONSUMER = 232, REGS_PRODUCER = 40;  // NWG > 1: 2 * 128 * 232 + 128 * 40 <= 65536
 };
+
+// points per CTA tile: 64 per consumer warpgroup; MODE 1 also needs a tangent row per point, held by the second
+// warpgroup in the fp16 engine and by the upper half of the tile in the TF32 engine
+template <int MODE, bool F16>
+constexpr int tile_points() {
+  return MODE != 1 ? Cfg<F16>::NWG * ROWS : (F16 ? ROWS : ROWS / 2);
+}
 
 // SIG: the geometry + tangent instantiation exchanges exp(100 z) between value and tangent rows
 template <bool F16, bool SIG>
@@ -133,6 +154,13 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   return d;
+}
+
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_arrive(uint32_t id, uint32_t threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -281,8 +309,8 @@ struct Params {
 
 }  // namespace tc
 
-// MODE 0: geometry.  MODE 1: geometry + tangent rows (rows 32..63 of a warpgroup tile carry d/d(ds) of rows 0..31).
-// MODE 2: colour.
+// MODE 0: geometry.  MODE 1: geometry + tangent rows d/d(ds) (fp16: warpgroup 1 holds the tangent rows of warpgroup 0's
+// points; TF32: rows 32..63 of the tile carry the tangents of rows 0..31).  MODE 2: colour.
 // F16 = false: 3xTF32 operands (mlp_engine 0).  F16 = true: fp16x3 operands (mlp_engine 2).
 template <int MODE, bool F16 = false>
 __global__ void __launch_bounds__(tc::Cfg<F16>::THREADS, 1) mlp_tc_kernel(const tc::Params prm) {
@@ -290,7 +318,10 @@ __global__ void __launch_bounds__(tc::Cfg<F16>::THREADS, 1) mlp_tc_kernel(const 
   using C = Cfg<F16>;
   using SmemLayout = SmemLayoutT<F16, MODE == 1>;
   constexpr int NWG = C::NWG, GR = C::GR, A_SUB = C::A_SUB, B_SUB = C::B_SUB;
-  constexpr int PTS = (MODE == 1) ? ROWS / 2 : ROWS;   // points per warpgroup tile
+  constexpr bool SPLIT = (MODE == 1) && F16;            // value and tangent rows in separate warpgroups
+  constexpr bool HALF_ROWS = (MODE == 1) && !SPLIT;     // rows 32..63 of a tile: the tangents of rows 0..31
+  constexpr int PTS = HALF_ROWS ? ROWS / 2 : ROWS;      // points per warpgroup tile
+  constexpr int TILE_PTS = tile_points<MODE, F16>();    // points per CTA tile
   extern __shared__ __align__(1024) char smem[];
   float* cst = reinterpret_cast<float*>(smem + SmemLayout::const_off);   // [n_layers][256] biases, then output rows
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SmemLayout::bar_off);
@@ -300,7 +331,7 @@ __global__ void __launch_bounds__(tc::Cfg<F16>::THREADS, 1) mlp_tc_kernel(const 
   const uint32_t b_base = smem_u32(smem + SmemLayout::b_off);
 
   const int tid = threadIdx.x;
-  const int64_t n_tiles = (prm.P + NWG * PTS - 1) / (NWG * PTS);   // a CTA tile = one tile per consumer warpgroup
+  const int64_t n_tiles = (prm.P + TILE_PTS - 1) / TILE_PTS;
   const FieldLayout& L = prm.lay;
   const int NL = prm.n_layers;
 
@@ -346,9 +377,15 @@ __global__ void __launch_bounds__(tc::Cfg<F16>::THREADS, 1) mlp_tc_kernel(const 
   const int wg = tid >> 7, t = tid & 127, warp = t >> 5, lane = t & 31;
   char* region = smem + SmemLayout::a_off + wg * C::A_REGION;
   const uint32_t a_base = smem_u32(region);
-  float* sig = reinterpret_cast<float*>(smem + SmemLayout::sig_off) + wg * SIG_FLOATS;
+  // SPLIT: the two exchange buffers, shared by both warpgroups
+  float* sig = reinterpret_cast<float*>(smem + SmemLayout::sig_off) + (SPLIT ? 0 : wg * SIG_FLOATS);
+  const bool tan_wg = SPLIT && wg == 1;        // every row of this warpgroup is a tangent row
   const uint32_t wg_bar = 1u + (uint32_t)wg;   // named barrier of this warpgroup (0 is __syncthreads)
-  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory"); };
+  auto wg_sync = [&]() { named_sync(wg_bar, 128); };
+  if (tan_wg) {   // both exchange buffers start empty
+    named_arrive(EX_EMPTY + 0, 256);
+    named_arrive(EX_EMPTY + 1, 256);
+  }
 
   float d[128];
 #pragma unroll
@@ -413,229 +450,283 @@ __global__ void __launch_bounds__(tc::Cfg<F16>::THREADS, 1) mlp_tc_kernel(const 
   const float* __restrict__ table = (MODE == 2) ? prm.tab.fc : prm.tab.fg;
 
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int64_t pbase = (tile * NWG + wg) * PTS;
+    const int64_t pbase = SPLIT ? tile * TILE_PTS : (tile * NWG + wg) * PTS;
     // every warp of the warpgroup has seen the previous tile's last MMAs complete before any of them overwrites the
     // first-layer ring, whose rows the whole warpgroup's MMAs read
     wg_sync();
-    {
-      // ===================================== layer 0: build + MMA =====================================
-      // two threads per row: half h owns features {8g + 4h + i : g < 4, i < 4} and writes columns [8h, 8h+8) of
-      // every first-layer slab (see tc_first_layer_map for the column order)
-      const int r = t & (ROWS - 1);
-      const int h = t >> 6;
-      const int64_t p = pbase + ((MODE == 1) ? (r & 31) : r);
-      const bool valid = p < prm.P;
-      const bool tangent = (MODE == 1) && (r >= 32);
-      uint32_t q = 0;   // first-layer slabs emitted
-      auto emit = [&](const float (&v)[8]) {
-        const uint32_t gq = q / GR;                  // GR consecutive slabs share a ring step
-        const uint32_t slot = gq % NA0;
-        char* a_dst = region + slot * (GR * A_SUB) + (q % GR) * A_SUB;
-        if constexpr (F16) store_a_half_f16(a_dst, r, h, v);
-        else store_a_half(a_dst, r, h, v);
-        ++q;
-        if (q % GR == 0) {
-          fence_proxy_async();
-          wg_sync();
-          step(a_base + slot * (GR * A_SUB), gq == 0);
-        }
-      };
-      // ---- gather + blend of this half's 16 features of code block fb (registers) ----
-      float feat[16];
-      float ds = 0.f;
-      // where this point's neighbour data lives (geometry modes: optionally indirected, see FieldIn::index)
-      const int64_t ps = (valid && MODE != 2) ? field_src(prm.in, p) : p;
-      if (valid) ds = prm.in.ds[ps];
-      auto gather = [&](int fb) {
+    // the tile's work for one role: TAN_WG = a SPLIT tangent warpgroup; the value warpgroup's layer 0 is MODE 0's.  The
+    // roles are separate instantiations, so neither carries the other's state through the register-bound build
+    auto tile_work = [&](auto tan_wg_c) {
+      constexpr bool TAN_WG = decltype(tan_wg_c)::value;
+      {
+        // ===================================== layer 0: build + MMA =====================================
+        // (TAN_WG: only the head block; the remaining first-layer steps are released unissued)
+        // two threads per row: half h owns features {8g + 4h + i : g < 4, i < 4} and writes columns [8h, 8h+8) of
+        // every first-layer slab (see tc_first_layer_map for the column order)
+        const int r = t & (ROWS - 1);
+        const int h = t >> 6;
+        const int64_t p = pbase + (HALF_ROWS ? (r & 31) : r);
+        const bool valid = p < prm.P;
+        const bool tangent = TAN_WG || (HALF_ROWS && r >= 32);
+        uint32_t q = 0;   // first-layer slabs emitted
+        auto emit = [&](const float (&v)[8]) {
+          const uint32_t gq = q / GR;                  // GR consecutive slabs share a ring step
+          const uint32_t slot = gq % NA0;
+          char* a_dst = region + slot * (GR * A_SUB) + (q % GR) * A_SUB;
+          if constexpr (F16) store_a_half_f16(a_dst, r, h, v);
+          else store_a_half(a_dst, r, h, v);
+          ++q;
+          if (q % GR == 0) {
+            fence_proxy_async();
+            wg_sync();
+            step(a_base + slot * (GR * A_SUB), gq == 0);
+          }
+        };
+        // ---- gather + blend of this half's 16 features of code block fb (registers) ----
+        float feat[16];
+        float ds = 0.f;
+        // where this point's neighbour data lives (geometry modes: optionally indirected, see FieldIn::index)
+        const int64_t ps = (valid && MODE != 2) ? field_src(prm.in, p) : p;
+        if (valid) ds = prm.in.ds[ps];
+        auto gather = [&](int fb) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) feat[i] = 0.f;
-        if (valid && !tangent) {
+          for (int i = 0; i < 16; ++i) feat[i] = 0.f;
+          if (valid && !tangent) {
 #pragma unroll
-          for (int k = 0; k < KNN_K; ++k) {
-            const int32_t sl = prm.in.slot[k * prm.in.stride + ps];
-            const float w = prm.in.w[k * prm.in.stride + ps];
-            const float* row = table + (int64_t)sl * Fdim + fb * FEAT + 4 * h;
+            for (int k = 0; k < KNN_K; ++k) {
+              const int32_t sl = prm.in.slot[k * prm.in.stride + ps];
+              const float w = prm.in.w[k * prm.in.stride + ps];
+              const float* row = table + (int64_t)sl * Fdim + fb * FEAT + 4 * h;
 #pragma unroll
-            for (int g4 = 0; g4 < 4; ++g4) {
-              const float4 a = __ldg(reinterpret_cast<const float4*>(row + 8 * g4));
-              feat[g4 * 4 + 0] = __fadd_rn(feat[g4 * 4 + 0], __fmul_rn(a.x, w));
-              feat[g4 * 4 + 1] = __fadd_rn(feat[g4 * 4 + 1], __fmul_rn(a.y, w));
-              feat[g4 * 4 + 2] = __fadd_rn(feat[g4 * 4 + 2], __fmul_rn(a.z, w));
-              feat[g4 * 4 + 3] = __fadd_rn(feat[g4 * 4 + 3], __fmul_rn(a.w, w));
+              for (int g4 = 0; g4 < 4; ++g4) {
+                const float4 a = __ldg(reinterpret_cast<const float4*>(row + 8 * g4));
+                feat[g4 * 4 + 0] = __fadd_rn(feat[g4 * 4 + 0], __fmul_rn(a.x, w));
+                feat[g4 * 4 + 1] = __fadd_rn(feat[g4 * 4 + 1], __fmul_rn(a.y, w));
+                feat[g4 * 4 + 2] = __fadd_rn(feat[g4 * 4 + 2], __fmul_rn(a.z, w));
+                feat[g4 * 4 + 3] = __fadd_rn(feat[g4 * 4 + 3], __fmul_rn(a.w, w));
+              }
             }
           }
-        }
-      };
-      gather(0);
-      // ---- head block: columns [0, off_feat): PE(ds) [, nabla, PE(view)], zero padded ----
-      {
-        float head[64];
+        };
+        gather(0);
+        // ---- head block: columns [0, off_feat): PE(ds) [, nabla, PE(view)], zero padded ----
+        {
+          float head[64];
 #pragma unroll
-        for (int i = 0; i < 64; ++i) head[i] = 0.f;
-        auto st = [&](int col, float v) { head[col] = v; };
-        if (valid) {
-          if (tangent) {
-            store_scalar_pe_tangent(ds, 0, L.Ld, st);
+          for (int i = 0; i < 64; ++i) head[i] = 0.f;
+          auto st = [&](int col, float v) { head[col] = v; };
+          if (valid) {
+            if (tangent) {
+              store_scalar_pe_tangent(ds, 0, L.Ld, st);
+            } else {
+              store_scalar_pe(ds, 0, L.Ld, st);
+              if (MODE == 2) {
+                float dx, dy, dz;
+                load_dir(prm.in, p, dx, dy, dz);
+                store_vec3_pe(dx, dy, dz, L.off_view, L.Lv, st);
+                if (L.use_nabla) {
+                  st(L.off_nabla + 0, prm.in.nabla[0 * prm.in.stride + p]);
+                  st(L.off_nabla + 1, prm.in.nabla[1 * prm.in.stride + p]);
+                  st(L.off_nabla + 2, prm.in.nabla[2 * prm.in.stride + p]);
+                }
+              }
+            }
+          }
+          for (int s = 0; s < off_feat / SLAB_K; ++s) {
+            float v[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = head[s * 16 + 8 * h + i];
+            emit(v);
+          }
+        }
+        for (int fb = 0; fb < (TAN_WG ? 0 : n_fb); ++fb) {   // (TAN_WG: the feature and band columns are zero)
+          if (fb > 0) gather(fb);
+          // ---- raw features: slab s holds groups g = 2s, 2s+1: columns [8h, 8h+8) = feat[2s][0..3], feat[2s+1][0..3] ----
+#pragma unroll
+          for (int s2 = 0; s2 < 2; ++s2) {
+            float v[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = feat[s2 * 8 + i];
+            emit(v);
+          }
+          // ---- bands: slab (b, g): columns [8h, 8h+8) = [sin(2^b f[g][0..3]), cos(2^b f[g][0..3])] ----
+          float fr = 1.f;
+          for (int b = 0; b < Lf; ++b) {
+#pragma unroll
+            for (int g4 = 0; g4 < 4; ++g4) {
+              float v[8];
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                float sn = 0.f, cs = 0.f;
+                if (valid && !tangent) sincosf(feat[g4 * 4 + i] * fr, &sn, &cs);
+                v[i] = sn;
+                v[4 + i] = cs;
+              }
+              emit(v);
+            }
+            fr *= 2.f;
+          }
+        }
+        if constexpr (GR > 1) {   // the first layer is padded with zero slabs (zero weights) to a whole number of steps
+          const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+          // (a tangent warpgroup only completes the step that holds the end of the head block)
+          while (TAN_WG ? q % GR != 0 : q < (uint32_t)prm.n_slabs[0]) emit(zero);
+        }
+        finish_layer();
+        if constexpr (TAN_WG) {
+          // the remaining first-layer steps would multiply exact zeros: not issued, but every weight slot is still
+          // released in ring order, and only after its FULL phase completed (the producer has then seen the slot's
+          // previous EMPTY phase complete, so this arrival counts in the phase of this step)
+          for (int s = (int)(q / GR); s < prm.n_slabs[0] / GR; ++s) {
+            const uint32_t sb = qb % NB;
+            mbar_wait(bar(B_FULL + sb), (qb / NB) & 1u);
+            if (lane == 0) mbar_arrive(bar(B_EMPTY + sb));
+            ++qb;
+          }
+        }
+      }
+
+      // ========================================== layers, epilogues ==========================================
+      const int cq = 2 * (lane & 3);              // first of this thread's two adjacent columns in every 8-column group
+      const int rr = 16 * warp + (lane >> 2);     // this thread's rows: rr and rr + 8
+      // accumulator values per epilogue chunk: column quarters, or eighths for the SPLIT exchange
+      constexpr int CH = SPLIT ? 16 : 32;
+      static_assert((128 / CH) % 2 == 0, "chunk qq of every layer uses exchange buffer qq % 2");
+      for (int l = 0; l < NL; ++l) {
+        if (l > 0) {
+          const int steps = prm.n_slabs[l] / GR;
+          for (int j = 0; j < steps; ++j) step(a_base + j * (GR * A_SUB), j == 0);
+          finish_layer();
+        }
+        const bool last = (l == NL - 1);
+        const float* bl = cst + l * MLP_W;
+        const float* wo = cst + NL * MLP_W;
+        float o[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+        for (int qq = 0; qq < 128 / CH; ++qq) {   // MODE 1 exchanges exp(100 z) one chunk at a time
+          // column of chunk value i: d[4 n8 + 2 hh + jj] holds column 8 n8 + cq + jj
+          auto col = [&](int i) { return 8 * ((CH * qq + i) >> 2) + cq + (i & 1); };
+          float v[CH];
+#pragma unroll
+          for (int i = 0; i < CH; ++i) v[i] = F16 ? d[CH * qq + i] * (1.0f / F16_W_SCALE) : d[CH * qq + i];
+          if (MODE == 2) {
+#pragma unroll
+            for (int i = 0; i < CH; ++i) v[i] = fmaxf(v[i] + bl[col(i)], 0.f);
+          } else if (MODE == 0) {
+#pragma unroll
+            for (int i = 0; i < CH; ++i) {
+              const float z = v[i] + bl[col(i)];
+              const float y = __log2f(1.0f + fast_exp2(z * K_EXP)) * K_LOG;
+              v[i] = z > 0.2f ? z : y;   // 100 z > 20
+            }
+          } else if constexpr (SPLIT) {
+            // warpgroup 0 (value rows) publishes e = exp(100 z) of eighth qq into buffer qq % 2 and keeps
+            // softplus = log(1 + e) / 100; warpgroup 1 (tangent rows: same fragment, same point) scales W t by
+            // sigma'(z) = e / (1 + e), then frees the buffer for eighth qq + 2
+            float* buf = sig + (qq & 1) * SIG_FLOATS;
+            if constexpr (!TAN_WG) {
+              named_sync(EX_EMPTY + (qq & 1), 256);
+#pragma unroll
+              for (int i = 0; i < CH; ++i) {
+                const float z = v[i] + bl[col(i)];
+                const float e = fast_exp2(z * K_EXP);
+                buf[i * 128 + t] = e;
+                v[i] = z > 0.2f ? z : __log2f(1.0f + e) * K_LOG;
+              }
+              named_arrive(EX_FULL + (qq & 1), 256);
+            } else {
+              named_sync(EX_FULL + (qq & 1), 256);
+#pragma unroll
+              for (int i = 0; i < CH; ++i) {
+                const float e = buf[i * 128 + t];
+                // 100 z > 20  <=>  e > exp(20)
+                v[i] *= e > 485165195.4097903f ? 1.f : __fdividef(e, e + 1.f);
+              }
+              named_arrive(EX_EMPTY + (qq & 1), 256);
+            }
           } else {
-            store_scalar_pe(ds, 0, L.Ld, st);
-            if (MODE == 2) {
-              float dx, dy, dz;
-              load_dir(prm.in, p, dx, dy, dz);
-              store_vec3_pe(dx, dy, dz, L.off_view, L.Lv, st);
-              if (L.use_nabla) {
-                st(L.off_nabla + 0, prm.in.nabla[0 * prm.in.stride + p]);
-                st(L.off_nabla + 1, prm.in.nabla[1 * prm.in.stride + p]);
-                st(L.off_nabla + 2, prm.in.nabla[2 * prm.in.stride + p]);
+            // MODE 1, TF32: value rows (warps 0, 1) publish e = exp(100 z); softplus = log(1 + e) / 100 for the value
+            // rows, sigma'(z) * (W t) with sigma' = e / (1 + e) for the tangent rows (warps 2, 3: same fragment, same
+            // point)
+            if (t < 64) {
+#pragma unroll
+              for (int i = 0; i < CH; ++i) {
+                const float z = v[i] + bl[col(i)];
+                const float e = fast_exp2(z * K_EXP);
+                sig[i * 64 + t] = e;
+                v[i] = z > 0.2f ? z : __log2f(1.0f + e) * K_LOG;
+              }
+            }
+            wg_sync();
+            if (t >= 64) {
+#pragma unroll
+              for (int i = 0; i < CH; ++i) {
+                const float e = sig[i * 64 + (t - 64)];
+                // 100 z > 20  <=>  e > exp(20)
+                v[i] *= e > 485165195.4097903f ? 1.f : __fdividef(e, e + 1.f);
+              }
+            }
+            wg_sync();   // the buffer is rewritten by the next quarter
+          }
+          if (!last) {
+#pragma unroll
+            for (int i = 0; i < CH; i += 2) store_a_pair<F16>(region, rr + 8 * ((i >> 1) & 1), col(i), v[i], v[i + 1]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < CH; ++i) {
+              const int c = col(i);
+              const int hh = (i >> 1) & 1;
+              o[hh][0] = fmaf(v[i], wo[c], o[hh][0]);
+              if (MODE == 2) {
+                o[hh][1] = fmaf(v[i], wo[MLP_W + c], o[hh][1]);
+                o[hh][2] = fmaf(v[i], wo[2 * MLP_W + c], o[hh][2]);
               }
             }
           }
         }
-        for (int s = 0; s < off_feat / SLAB_K; ++s) {
-          float v[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = head[s * 16 + 8 * h + i];
-          emit(v);
-        }
-      }
-      for (int fb = 0; fb < n_fb; ++fb) {
-        if (fb > 0) gather(fb);
-        // ---- raw features: slab s holds groups g = 2s, 2s+1: columns [8h, 8h+8) = feat[g = 2s][0..3], feat[2s+1][0..3] ----
-#pragma unroll
-        for (int s2 = 0; s2 < 2; ++s2) {
-          float v[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = feat[s2 * 8 + i];
-          emit(v);
-        }
-        // ---- bands: slab (b, g): columns [8h, 8h+8) = [sin(2^b f[g][0..3]), cos(2^b f[g][0..3])] ----
-        float fr = 1.f;
-        for (int b = 0; b < Lf; ++b) {
-#pragma unroll
-          for (int g4 = 0; g4 < 4; ++g4) {
-            float v[8];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float sn = 0.f, cs = 0.f;
-              if (valid && !tangent) sincosf(feat[g4 * 4 + i] * fr, &sn, &cs);
-              v[i] = sn;
-              v[4 + i] = cs;
-            }
-            emit(v);
-          }
-          fr *= 2.f;
-        }
-      }
-      if constexpr (GR > 1) {   // the first layer is padded with zero slabs (zero weights) to a whole number of steps
-        const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        while (q < (uint32_t)prm.n_slabs[0]) emit(zero);
-      }
-      finish_layer();
-    }
-
-    // ========================================== layers, epilogues ==========================================
-    const int cq = 2 * (lane & 3);              // first of this thread's two adjacent columns in every 8-column group
-    const int rr = 16 * warp + (lane >> 2);     // this thread's rows: rr and rr + 8
-    for (int l = 0; l < NL; ++l) {
-      if (l > 0) {
-        const int steps = prm.n_slabs[l] / GR;
-        for (int j = 0; j < steps; ++j) step(a_base + j * (GR * A_SUB), j == 0);
-        finish_layer();
-      }
-      const bool last = (l == NL - 1);
-      const float* bl = cst + l * MLP_W;
-      const float* wo = cst + NL * MLP_W;
-      float o[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-#pragma unroll
-      for (int qq = 0; qq < 4; ++qq) {   // column quarters: MODE 1 exchanges exp(100 z) one quarter at a time
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = F16 ? d[32 * qq + i] * (1.0f / F16_W_SCALE) : d[32 * qq + i];
-        if (MODE == 2) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i] + bl[8 * (8 * qq + (i >> 2)) + cq + (i & 1)], 0.f);
-        } else if (MODE == 0) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float z = v[i] + bl[8 * (8 * qq + (i >> 2)) + cq + (i & 1)];
-            const float y = __log2f(1.0f + fast_exp2(z * K_EXP)) * K_LOG;
-            v[i] = z > 0.2f ? z : y;   // 100 z > 20
-          }
-        } else {
-          // MODE 1: value rows (warps 0, 1) publish e = exp(100 z); softplus = log(1 + e) / 100 for the value rows,
-          // sigma'(z) * (W t) with sigma' = e / (1 + e) for the tangent rows (warps 2, 3: same fragment, same point)
-          if (t < 64) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float z = v[i] + bl[8 * (8 * qq + (i >> 2)) + cq + (i & 1)];
-              const float e = fast_exp2(z * K_EXP);
-              sig[i * 64 + t] = e;
-              v[i] = z > 0.2f ? z : __log2f(1.0f + e) * K_LOG;
-            }
-          }
-          wg_sync();
-          if (t >= 64) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float e = sig[i * 64 + (t - 64)];
-              // 100 z > 20  <=>  e > exp(20)
-              v[i] *= e > 485165195.4097903f ? 1.f : __fdividef(e, e + 1.f);
-            }
-          }
-          wg_sync();   // the buffer is rewritten by the next quarter
-        }
         if (!last) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const int col = 8 * (8 * qq + (i >> 2)) + cq;
-            store_a_pair<F16>(region, rr + 8 * ((i >> 1) & 1), col, v[i], v[i + 1]);
-          }
+          fence_proxy_async();
+          wg_sync();   // the next layer's A operand is complete
         } else {
+          // the four threads of a quad hold the partial dot products of the same two rows
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int col = 8 * (8 * qq + (i >> 2)) + cq + (i & 1);
-            const int hh = (i >> 1) & 1;
-            o[hh][0] = fmaf(v[i], wo[col], o[hh][0]);
-            if (MODE == 2) {
-              o[hh][1] = fmaf(v[i], wo[MLP_W + col], o[hh][1]);
-              o[hh][2] = fmaf(v[i], wo[2 * MLP_W + col], o[hh][2]);
+          for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+              o[hh][k] += __shfl_xor_sync(0xffffffffu, o[hh][k], 1);
+              o[hh][k] += __shfl_xor_sync(0xffffffffu, o[hh][k], 2);
+            }
+          if ((lane & 3) == 0) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int row = rr + 8 * hh;
+              const int64_t p = pbase + (HALF_ROWS ? (row & 31) : row);
+              if (p >= prm.P) continue;
+              if (MODE == 2) {
+                prm.out0[0 * prm.in.stride + p] = sigmoid_acc(o[hh][0] + __ldg(prm.b_out + 0));
+                prm.out0[1 * prm.in.stride + p] = sigmoid_acc(o[hh][1] + __ldg(prm.b_out + 1));
+                prm.out0[2 * prm.in.stride + p] = sigmoid_acc(o[hh][2] + __ldg(prm.b_out + 2));
+              } else if (MODE == 0 || (SPLIT ? !TAN_WG : row < 32)) {
+                prm.out0[p] = o[hh][0] + __ldg(prm.b_out);
+              } else if (prm.out1) {
+                const int64_t ps = field_src(prm.in, p);
+                prm.out1[0 * prm.in.stride + p] = o[hh][0] * prm.in.grad[0 * prm.in.stride + ps];
+                prm.out1[1 * prm.in.stride + p] = o[hh][0] * prm.in.grad[1 * prm.in.stride + ps];
+                prm.out1[2 * prm.in.stride + p] = o[hh][0] * prm.in.grad[2 * prm.in.stride + ps];
+              }
             }
           }
         }
       }
-      if (!last) {
-        fence_proxy_async();
-        wg_sync();   // the next layer's A operand is complete
-      } else {
-        // the four threads of a quad hold the partial dot products of the same two rows
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int k = 0; k < 3; ++k) {
-            o[hh][k] += __shfl_xor_sync(0xffffffffu, o[hh][k], 1);
-            o[hh][k] += __shfl_xor_sync(0xffffffffu, o[hh][k], 2);
-          }
-        if ((lane & 3) == 0) {
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int row = rr + 8 * hh;
-            const int64_t p = pbase + ((MODE == 1) ? (row & 31) : row);
-            if (p >= prm.P) continue;
-            if (MODE == 2) {
-              prm.out0[0 * prm.in.stride + p] = sigmoid_acc(o[hh][0] + __ldg(prm.b_out + 0));
-              prm.out0[1 * prm.in.stride + p] = sigmoid_acc(o[hh][1] + __ldg(prm.b_out + 1));
-              prm.out0[2 * prm.in.stride + p] = sigmoid_acc(o[hh][2] + __ldg(prm.b_out + 2));
-            } else if (MODE == 0 || row < 32) {
-              prm.out0[p] = o[hh][0] + __ldg(prm.b_out);
-            } else if (prm.out1) {
-              const int64_t ps = field_src(prm.in, p);
-              prm.out1[0 * prm.in.stride + p] = o[hh][0] * prm.in.grad[0 * prm.in.stride + ps];
-              prm.out1[1 * prm.in.stride + p] = o[hh][0] * prm.in.grad[1 * prm.in.stride + ps];
-              prm.out1[2 * prm.in.stride + p] = o[hh][0] * prm.in.grad[2 * prm.in.stride + ps];
-            }
-          }
-        }
-      }
-    }
+    };
+    if (tan_wg) tile_work(std::true_type{});
+    else tile_work(std::false_type{});
+  }
+  // the tangent warpgroup's last two EMPTY arrivals have no matching wait yet: take them, so that no named barrier is
+  // left part-way through a phase when the CTA exits
+  if (SPLIT && wg == 0) {
+    named_sync(EX_EMPTY + 0, 256);
+    named_sync(EX_EMPTY + 1, 256);
   }
 }
 
@@ -772,13 +863,12 @@ static int launch_tc(const nmb_field* f, const MlpFfma& fm, const MlpTc& tm, con
   prm.out0 = out0;
   prm.out1 = out1;
   using C = tc::Cfg<F16>;
-  constexpr int PTS = (MODE == 1) ? tc::ROWS / 2 : tc::ROWS;
   const size_t smem = tc::SmemLayoutT<F16, MODE == 1>::total;
   static DeviceOnce attr_once;
   NMB_CUDA_OK(attr_once.run([&] {
     return cudaFuncSetAttribute(mlp_tc_kernel<MODE, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }));
-  const int64_t tiles = ceil_div(P, (int64_t)C::NWG * PTS);
+  const int64_t tiles = ceil_div(P, (int64_t)tc::tile_points<MODE, F16>());
   const int64_t grid = tiles < (int64_t)sm_count() ? tiles : (int64_t)sm_count();
   ProfScope prof(MODE == 2 ? PROF_COLOR : (MODE == 1 ? PROF_GEO_JVP : PROF_GEO), P, stream);
   mlp_tc_kernel<MODE, F16><<<(unsigned)grid, C::THREADS, smem, stream>>>(prm);
