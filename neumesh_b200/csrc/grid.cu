@@ -17,22 +17,12 @@
 #include <math_constants.h>
 
 #include <algorithm>
-#include <cstdlib>
 #include <vector>
 
 #include "grid.cuh"
-#include "knn_coop.cuh"
 #include "knn_walk.cuh"
 
 namespace nmb {
-
-// The directory start of the thread-per-query walk is compiled in only with -DNMB_KNN_DIRECTORY=1: it is bit-identical
-// and was not faster when measured, and merely carrying its code raises the bound scan's register count (66 -> 75 per
-// thread), so the shipped build leaves it out.
-#ifndef NMB_KNN_DIRECTORY
-#define NMB_KNN_DIRECTORY 0
-#endif
-#define NMB_GV_ARG(gv) (NMB_KNN_DIRECTORY ? &(gv) : nullptr)
 
 // ------------------------------------------------------------------------------------------------------------
 // build
@@ -248,29 +238,6 @@ __global__ void lvl_boxes_kernel(int32_t first_node, int32_t n_nodes, const int3
   nodes[NODE_F4 * n + 3] = make_float4(ux, uy, uz, th);
 }
 
-
-// Directory tables of the cooperative walk (knn_coop.cuh).  One thread per octree node of depth `depth`: a node AT a
-// directory level fills its own cell; a LEAF above a directory level fills every cell it covers at that level.
-__global__ void dir_fill_kernel(int32_t first_node, int32_t n_nodes, int depth, int L, const uint32_t* __restrict__ code,
-                                const int32_t* __restrict__ nbegin, const int32_t* __restrict__ nfirst, int lmin, int lmax,
-                                const int32_t* __restrict__ dir_off /*[lmax - lmin + 1] on device*/,
-                                int32_t* __restrict__ dir) {
-  const int32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_nodes) return;
-  const int32_t n = first_node + t;
-  const uint32_t prefix = depth == 0 ? 0u : (code[nbegin[n]] >> (3 * (L - depth)));
-  const bool leaf = nfirst[n] < 0;
-  for (int l = max(lmin, depth); l <= lmax; ++l) {
-    if (l == depth) {
-      dir[dir_off[l - lmin] + prefix] = n;
-    } else if (leaf) {
-      const int sh = 3 * (l - depth);
-      const uint32_t b = prefix << sh, e = (prefix + 1u) << sh;
-      for (uint32_t c = b; c < e; ++c) dir[dir_off[l - lmin] + c] = n;
-    }
-  }
-}
-
 static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb_grid* g) {
   NMB_CHECK(V >= KNN_K, "mesh needs at least 8 vertices");
   NMB_CHECK(V < (int64_t(1) << 30), "too many vertices");
@@ -342,9 +309,7 @@ static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb
   NMB_LAUNCH_OK();
 
   // level-by-level subdivision
-  // leaf capacity (points per leaf): tunable for experiments, default LEAF_MAX
-  const int leaf_max = getenv("NMB_LEAF_MAX") ? std::max(1, atoi(getenv("NMB_LEAF_MAX"))) : LEAF_MAX;
-  const int64_t cap = V + (int64_t)(L + 1) * (V / (leaf_max + 1) + 1) + 16;
+  const int64_t cap = V + (int64_t)(L + 1) * (V / (LEAF_MAX + 1) + 1) + 16;
   StreamBuf node_b, point_b;   // 4 node arrays of `cap` entries; 4 per-point arrays
   NMB_CUDA_OK(node_b.alloc(sizeof(int32_t) * 4 * cap, stream));
   NMB_CUDA_OK(point_b.alloc(sizeof(int32_t) * (4 * V + 4), stream));
@@ -365,7 +330,7 @@ static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb
     NMB_CUDA_OK(cudaMemcpyAsync(nfirst.p, &root[2], 4, cudaMemcpyHostToDevice, stream));
     NMB_CUDA_OK(cudaMemcpyAsync(nlast.p, &root[3], 4, cudaMemcpyHostToDevice, stream));
     // all points start in the root (V >= 8 > ... root splits iff V > LEAF_MAX and L > 0)
-    int fill = (V > leaf_max && L > 0) ? 0 : -1;
+    int fill = (V > LEAF_MAX && L > 0) ? 0 : -1;
     NMB_CUDA_OK(cudaMemsetAsync(pnode.p, fill == 0 ? 0 : 0xff, sizeof(int32_t) * V, stream));
   }
   int32_t n_nodes = 1;
@@ -387,7 +352,7 @@ static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb
                                                                  nbegin.p, nend.p, nfirst.p, nlast.p, newnode.p);
     NMB_LAUNCH_OK();
     lvl_activate_kernel<<<(unsigned)blocks, threads, 0, stream>>>(newnode.p, nbegin.p, nend.p, V, (l + 1 < L) ? 1 : 0,
-                                                                   leaf_max, pnode.p);
+                                                                   LEAF_MAX, pnode.p);
     NMB_LAUNCH_OK();
     n_nodes += n_new;
     lvl_off.push_back(n_nodes);
@@ -402,56 +367,8 @@ static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb
                                                                                nlast.p, g->pts.p, g->nodes.p);
     NMB_LAUNCH_OK();
   }
-  // directory tables: levels [3, min(L - 1, 7)] (finer cells than the vertex spacing buy nothing).  OPT-IN
-  // (build with -DNMB_KNN_DIRECTORY=1 and set NMB_KNN_DIR=1; the cooperative kernels, NMB_KNN_COOP=1, use it too): the
-  // directory start is bit-identical but was not faster when measured: with a warm bound the ball meets only 1-2
-  // children per TOP level, so the levels it skips cost about as much as the 2x2x2-cell seeding does; the expansions that
-  // dominate a walk sit at the bottom levels, where cells are as small as the ball.
-  g->dir_lmin = 3;
-  g->dir_lmax = std::min(L - 1, 7);
-  if (getenv("NMB_KNN_DIR_MAX")) g->dir_lmax = std::min(g->dir_lmax, atoi(getenv("NMB_KNN_DIR_MAX")));
-  static const bool want_dir = (NMB_KNN_DIRECTORY && getenv("NMB_KNN_DIR") != nullptr) || getenv("NMB_KNN_COOP") != nullptr;
-  if (!want_dir) g->dir_lmax = g->dir_lmin - 1;
-  if (g->dir_lmax >= g->dir_lmin) {
-    int64_t total = 0;
-    int32_t offs[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int l = g->dir_lmin; l <= g->dir_lmax; ++l) {
-      offs[l - g->dir_lmin] = (int32_t)total;
-      g->dir_off[l - g->dir_lmin] = (int32_t)total;
-      total += int64_t(1) << (3 * l);
-    }
-    NMB_CUDA_OK(g->dir.alloc(total));
-    NMB_CUDA_OK(cudaMemsetAsync(g->dir.p, 0xff, sizeof(int32_t) * total, stream));
-    StreamBuf offs_dev;
-    NMB_CUDA_OK(offs_dev.alloc(sizeof(offs), stream));
-    NMB_CUDA_OK(cudaMemcpyAsync(offs_dev.p, offs, sizeof(offs), cudaMemcpyHostToDevice, stream));
-    for (int dpt = 0; dpt + 1 < (int)lvl_off.size() && dpt <= g->dir_lmax; ++dpt) {
-      const int32_t first = lvl_off[dpt], cnt = lvl_off[dpt + 1] - lvl_off[dpt];
-      if (cnt <= 0) continue;
-      dir_fill_kernel<<<(unsigned)ceil_div(cnt, threads), threads, 0, stream>>>(
-          first, cnt, dpt, L, code.p, nbegin.p, nfirst.p, g->dir_lmin, g->dir_lmax, offs_dev.as<int32_t>(), g->dir.p);
-      NMB_LAUNCH_OK();
-    }
-    NMB_CUDA_OK(cudaStreamSynchronize(stream));   // `offs` is a stack array
-  }
   NMB_CUDA_OK(cudaStreamSynchronize(stream));
   return 0;
-}
-
-GridView make_view(const nmb_grid* g) {
-  GridView v{};
-  v.nodes = g->nodes.p;
-  v.pts = g->pts.p;
-  static const bool no_dir = getenv("NMB_KNN_NO_DIR") != nullptr;
-  v.dir = (g->dir_lmax >= g->dir_lmin && !no_dir) ? g->dir.p : nullptr;
-  v.dir_lmin = g->dir_lmin;
-  v.dir_lmax = v.dir ? g->dir_lmax : g->dir_lmin - 1;
-  v.bmin[0] = g->bmin[0];
-  v.bmin[1] = g->bmin[1];
-  v.bmin[2] = g->bmin[2];
-  v.inv_cell = g->inv_cell;
-  v.levels = g->levels;
-  return v;
 }
 
 __device__ __forceinline__ void load_query(const PointSrc& src, int64_t p, float& qx, float& qy, float& qz) {
@@ -505,18 +422,9 @@ __device__ __forceinline__ void mesh_distance_point(const float4* __restrict__ p
   }
 }
 
-__global__ void __launch_bounds__(128)
-knn_distance_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts,
-                    const float4* __restrict__ indicator, float w1, PointSrc src, int64_t P, KnnOut out) {
-  const int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (p >= P) return;
-  float qx, qy, qz;
-  load_query(src, p, qx, qy, qz);
-  float d2[KNN_K];
-  int32_t ix[KNN_K];
-  knn_walk<KNN_K, false>(nodes, pts, qx, qy, qz, d2, ix);
-  float w[KNN_K], ds, grad[3];
-  mesh_distance_point(pts, indicator, w1, qx, qy, qz, d2, ix, w, ds, grad);
+// one query's results into the SoA arrays of `out` (element (k, p) at [k * stride + p])
+__device__ __forceinline__ void store_knn_out(const KnnOut& out, int64_t p, float ds, const int32_t (&ix)[KNN_K],
+                                              const float (&w)[KNN_K], const float (&grad)[3]) {
   out.ds[p] = ds;
 #pragma unroll
   for (int k = 0; k < KNN_K; ++k) {
@@ -530,13 +438,27 @@ knn_distance_kernel(const float4* __restrict__ nodes, const float4* __restrict__
   }
 }
 
+__global__ void __launch_bounds__(128)
+knn_distance_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts,
+                    const float4* __restrict__ indicator, float w1, PointSrc src, int64_t P, KnnOut out) {
+  const int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  float qx, qy, qz;
+  load_query(src, p, qx, qy, qz);
+  float d2[KNN_K];
+  int32_t ix[KNN_K];
+  knn_walk<KNN_K, false>(nodes, pts, qx, qy, qz, d2, ix);
+  float w[KNN_K], ds, grad[3];
+  mesh_distance_point(pts, indicator, w1, qx, qy, qz, d2, ix, w, ds, grad);
+  store_knn_out(out, p, ds, ix, w, grad);
+}
+
 // Ray-ordered variant: one thread per RAY walks its S samples in depth order and warm-starts every query with the
 // previous sample's neighbours (consecutive samples are <~0.03 apart, so the initial 8th-best bound is already within
 // a few percent of the final one and the octree walk prunes almost everything).  A warp = 32 neighbouring rays.
-template <int MINB, int ORDER>
-__global__ void __launch_bounds__(128, MINB)
+__global__ void __launch_bounds__(128, 10)
 knn_rays_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts, const float4* __restrict__ indicator,
-                float w1, PointSrc src, int S, int seg, KnnOut out, const GridView gv) {
+                float w1, PointSrc src, int S, int seg, KnnOut out) {
   // thread t handles samples [g * seg, (g + 1) * seg) of ray r, t = g * R + r: with few rays (multi-GPU shards) a
   // ray's samples are split over several threads so that the launch still fills the GPU (one cold walk per segment)
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -560,26 +482,16 @@ knn_rays_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts
 #pragma unroll
       for (int k = 0; k < KNN_K; ++k) ix[k] = src.seed_slot[k * src.seed_stride + sp0];
       warm_rerank<KNN_K>(pts, qx, qy, qz, d2, ix);
-      knn_walk<KNN_K, true, ORDER>(nodes, pts, qx, qy, qz, d2, ix, NMB_GV_ARG(gv));
+      knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix);
     } else if (s == s_begin) {
-      knn_walk<KNN_K, false, ORDER>(nodes, pts, qx, qy, qz, d2, ix);
+      knn_walk<KNN_K, false>(nodes, pts, qx, qy, qz, d2, ix);
     } else {
       warm_rerank<KNN_K>(pts, qx, qy, qz, d2, ix);
-      knn_walk<KNN_K, true, ORDER>(nodes, pts, qx, qy, qz, d2, ix, NMB_GV_ARG(gv));
+      knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix);
     }
     float w[KNN_K], ds, grad[3];
     mesh_distance_point(pts, indicator, w1, qx, qy, qz, d2, ix, w, ds, grad);
-    out.ds[p] = ds;
-#pragma unroll
-    for (int k = 0; k < KNN_K; ++k) {
-      out.slot[k * out.stride + p] = ix[k];
-      out.w[k * out.stride + p] = w[k];
-    }
-    if (out.grad) {
-      out.grad[0 * out.stride + p] = grad[0];
-      out.grad[1 * out.stride + p] = grad[1];
-      out.grad[2 * out.stride + p] = grad[2];
-    }
+    store_knn_out(out, p, ds, ix, w, grad);
   }
 }
 
@@ -589,7 +501,7 @@ knn_rays_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts
 __global__ void __launch_bounds__(128)
 knn_lists_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts, const float4* __restrict__ indicator,
                  float w1, const float* __restrict__ xyz, const int32_t* __restrict__ off,
-                 const int32_t* __restrict__ cnt, int64_t R, int seg, int max_seg, KnnOut out, const GridView gv) {
+                 const int32_t* __restrict__ cnt, int64_t R, int seg, int max_seg, KnnOut out) {
   // thread t = g * R + r handles entries [g * seg, (g + 1) * seg) of ray r's list (short serial chains)
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t r = t % R;
@@ -607,230 +519,18 @@ knn_lists_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pt
       knn_walk<KNN_K, false>(nodes, pts, qx, qy, qz, d2, ix);
     } else {
       warm_rerank<KNN_K>(pts, qx, qy, qz, d2, ix);
-      knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix, NMB_GV_ARG(gv));
+      knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix);
     }
     float w[KNN_K], ds, grad[3];
     mesh_distance_point(pts, indicator, w1, qx, qy, qz, d2, ix, w, ds, grad);
-    out.ds[p] = ds;
-#pragma unroll
-    for (int k = 0; k < KNN_K; ++k) {
-      out.slot[k * out.stride + p] = ix[k];
-      out.w[k * out.stride + p] = w[k];
-    }
-    if (out.grad) {
-      out.grad[0 * out.stride + p] = grad[0];
-      out.grad[1 * out.stride + p] = grad[1];
-      out.grad[2 * out.stride + p] = grad[2];
-    }
+    store_knn_out(out, p, ds, ix, w, grad);
   }
 }
-
-
-// ------------------------------------------------------------------------------------------------------------
-// group-cooperative kernels (knn_coop.cuh): 8 lanes per query chain, 16 chains per 128-thread block
-// ------------------------------------------------------------------------------------------------------------
-static bool knn_legacy() {
-  // Default: thread-per-query kernels (with the directory start).  NMB_KNN_COOP=1 selects the 8-lanes-per-query
-  // cooperative kernels instead: bit-identical results, but they issue about twice the warp instructions per query
-  // (shuffles, ranking, serial insertions) and were measured slower; kept as an independent implementation for
-  // cross-checks.
-  static const bool v = getenv("NMB_KNN_COOP") == nullptr;
-  return v;
-}
-
-#define NMB_COOP_PROLOGUE()                                                                    \
-  __shared__ uint32_t stack_mem[coop::GROUPS_PER_BLOCK * coop::STACK_WORDS];                   \
-  const coop::Lane ln = coop::make_lane();                                                     \
-  uint32_t* stk = stack_mem + (threadIdx.x / coop::G) * coop::STACK_WORDS;                     \
-  const int32_t root_link = __float_as_int(__ldg(&gv.nodes[0]).w);                             \
-  const int32_t root_cnt = __float_as_int(__ldg(&gv.nodes[1]).w);                              \
-  const int64_t chain = blockIdx.x * (int64_t)coop::GROUPS_PER_BLOCK + threadIdx.x / coop::G;
-
-// explicit points or ray samples in any order: one cold query per group
-template <int MINB>
-__global__ void __launch_bounds__(coop::BLOCK, MINB)
-knn_points_coop_kernel(GridView gv, const float4* __restrict__ indicator, float w1, PointSrc src, int64_t P, KnnOut out) {
-  NMB_COOP_PROLOGUE()
-  if (chain >= P) return;
-  float qx, qy, qz;
-  load_query(src, chain, qx, qy, qz);
-  float d;
-  int32_t ix;
-  coop::query(gv, ln, stk, root_link, root_cnt, indicator, w1, qx, qy, qz, false, d, ix, out, chain);
-}
-
-// ray-ordered: chain t = g * R + r walks samples [g * seg, (g + 1) * seg) of ray r in depth order, every query
-// warm-started with the previous sample's neighbours; the 4 chains of a warp are 4 neighbouring rays
-template <int MINB>
-__global__ void __launch_bounds__(coop::BLOCK, MINB)
-knn_rays_coop_kernel(GridView gv, const float4* __restrict__ indicator, float w1, PointSrc src, int S, int seg, KnnOut out) {
-  NMB_COOP_PROLOGUE()
-  const int64_t r = chain % src.R;
-  const int s_begin = (int)(chain / src.R) * seg;
-  if (s_begin >= S) return;
-  const int s_end = min(s_begin + seg, S);
-  const float ox = src.rays_o[r * 3 + 0], oy = src.rays_o[r * 3 + 1], oz = src.rays_o[r * 3 + 2];
-  const float dx = src.rays_d[r * 3 + 0], dy = src.rays_d[r * 3 + 1], dz = src.rays_d[r * 3 + 2];
-  float d;
-  int32_t ix;
-  for (int s = s_begin; s < s_end; ++s) {
-    const int64_t p = (int64_t)s * src.R + r;
-    const float z = src.z[p];
-    const float qx = __fadd_rn(ox, __fmul_rn(z, dx));
-    const float qy = __fadd_rn(oy, __fmul_rn(z, dy));
-    const float qz = __fadd_rn(oz, __fmul_rn(z, dz));
-    coop::query(gv, ln, stk, root_link, root_cnt, indicator, w1, qx, qy, qz, s != s_begin, d, ix, out, p);
-  }
-}
-
-// per-ray lists of explicit points (the compacted live samples of nmb_render): chain t = g * R + r handles entries
-// [g * seg, (g + 1) * seg) of ray r's list
-template <int MINB>
-__global__ void __launch_bounds__(coop::BLOCK, MINB)
-knn_lists_coop_kernel(GridView gv, const float4* __restrict__ indicator, float w1, const float* __restrict__ xyz,
-                      const int32_t* __restrict__ off, const int32_t* __restrict__ cnt, int64_t R, int seg, int max_seg,
-                      KnnOut out) {
-  NMB_COOP_PROLOGUE()
-  const int64_t r = chain % R;
-  const int gseg = (int)(chain / R);
-  if (gseg >= max_seg) return;
-  const int64_t b = off[r];
-  const int j_begin = gseg * seg;
-  const int n = min(cnt[r], j_begin + seg);
-  float d;
-  int32_t ix;
-  for (int j = j_begin; j < n; ++j) {
-    const int64_t p = b + j;
-    const float qx = xyz[p * 3], qy = xyz[p * 3 + 1], qz = xyz[p * 3 + 2];
-    coop::query(gv, ln, stk, root_link, root_cnt, indicator, w1, qx, qy, qz, j != j_begin, d, ix, out, p);
-  }
-}
-
-// bounded near / far, every sample evaluated (small launches): one cold query per group
-template <int MINB>
-__global__ void __launch_bounds__(coop::BLOCK, MINB)
-bound_scan_coop_kernel(GridView gv, const float4* __restrict__ indicator, float w1, const float* __restrict__ rays_o,
-                       const float* __restrict__ dirs, const float* __restrict__ near, const float* __restrict__ far,
-                       int64_t R, int n_grid, float thresh, int32_t* __restrict__ bnear, int32_t* __restrict__ bfar) {
-  NMB_COOP_PROLOGUE()
-  if (chain >= R * n_grid) return;
-  const int64_t r = chain % R;
-  const int s = (int)(chain / R);
-  const float t = linspace01(s, n_grid);
-  const float dep = __fadd_rn(__fmul_rn(near[r], __fsub_rn(1.0f, t)), __fmul_rn(far[r], t));  // renderer.py:81
-  const float qx = __fadd_rn(rays_o[r * 3 + 0], __fmul_rn(dep, dirs[r * 3 + 0]));
-  const float qy = __fadd_rn(rays_o[r * 3 + 1], __fmul_rn(dep, dirs[r * 3 + 1]));
-  const float qz = __fadd_rn(rays_o[r * 3 + 2], __fmul_rn(dep, dirs[r * 3 + 2]));
-  float d;
-  int32_t ix;
-  const float ds = coop::query(gv, ln, stk, root_link, root_cnt, indicator, w1, qx, qy, qz, false, d, ix, KnnOut{}, 0);
-  if (ds < thresh && ln.gl == 0) {
-    atomicMin(&bnear[r], __float_as_int(dep));
-    atomicMax(&bfar[r], __float_as_int(dep));
-  }
-}
-
-// ray-ordered bounded near / far with early exit and the shell certificate (same logic as bound_rays_kernel below):
-// chain t = g * R + r scans samples [g * BOUND_SEG, (g + 1) * BOUND_SEG) of ray r from the front to its first hit and
-// from the back to its last hit
-constexpr int BOUND_SEG_COOP = 32;
-template <int MINB>
-__global__ void __launch_bounds__(coop::BLOCK, MINB)
-bound_rays_coop_kernel(GridView gv, const float4* __restrict__ indicator, float w1, const float* __restrict__ rays_o,
-                       const float* __restrict__ dirs, const float* __restrict__ near, const float* __restrict__ far,
-                       int64_t R, int n_grid, float thresh, int32_t* __restrict__ bnear, int32_t* __restrict__ bfar,
-                       ShellGrid shell) {
-  NMB_COOP_PROLOGUE()
-  const int64_t r = chain % R;
-  const int s_begin = (int)(chain / R) * BOUND_SEG_COOP;
-  if (s_begin >= n_grid) return;
-  const int s_end = min(s_begin + BOUND_SEG_COOP, n_grid);
-  const float ox = rays_o[r * 3 + 0], oy = rays_o[r * 3 + 1], oz = rays_o[r * 3 + 2];
-  const float dx = dirs[r * 3 + 0], dy = dirs[r * 3 + 1], dz = dirs[r * 3 + 2];
-  const float nr = near[r], fr = far[r];
-  float d;
-  int32_t ix;
-  bool have_prev = false;   // the lanes hold the neighbours of some earlier sample of this ray (valid warm start)
-  // mesh distance at sample s, or +inf / -inf when the sample lies in a cell certified outside / inside the shell
-  auto ds_at = [&](int s, float& depth) {
-    const float tt = linspace01(s, n_grid);
-    depth = __fadd_rn(__fmul_rn(nr, __fsub_rn(1.0f, tt)), __fmul_rn(fr, tt));  // renderer.py:81
-    const float qx = __fadd_rn(ox, __fmul_rn(depth, dx));
-    const float qy = __fadd_rn(oy, __fmul_rn(depth, dy));
-    const float qz = __fadd_rn(oz, __fmul_rn(depth, dz));
-    if (shell.cells) {
-      const float sc = 0.5f * (float)shell.G / shell.B;
-      const float fx = (qx + shell.B) * sc, fy = (qy + shell.B) * sc, fz = (qz + shell.B) * sc;
-      if (fx >= 0.f && fy >= 0.f && fz >= 0.f && fx < (float)shell.G && fy < (float)shell.G && fz < (float)shell.G) {
-        const int64_t cell = ((int64_t)(int)fz * shell.G + (int)fy) * shell.G + (int)fx;
-        const uint8_t code = __ldg(shell.cells + cell);
-        if (code == 1) return CUDART_INF_F;    // proven outside the shell: mask false
-        if (code == 2) return -CUDART_INF_F;   // proven inside the shell: mask true (only the depth matters)
-      } else {
-        const float ex = qx - shell.cx, ey = qy - shell.cy, ez = qz - shell.cz;
-        if (ex * ex + ey * ey + ez * ez >= shell.far_r * shell.far_r) return CUDART_INF_F;
-      }
-    }
-    const bool warm = have_prev;
-    have_prev = true;
-    return coop::query(gv, ln, stk, root_link, root_cnt, indicator, w1, qx, qy, qz, warm, d, ix, KnnOut{}, 0);
-  };
-  int first = -1;
-  float depth = 0.f;
-  for (int s = s_begin; s < s_end; ++s) {
-    if (ds_at(s, depth) < thresh) {
-      first = s;
-      if (ln.gl == 0) atomicMin(&bnear[r], __float_as_int(depth));   // depths are >= 0: bit patterns order like values
-      break;
-    }
-  }
-  if (first < 0) return;  // no hit in this segment
-  for (int s = s_end - 1; s >= first; --s) {
-    if (s == first) {   // known to be a hit: the loop always terminates with a far candidate
-      if (ln.gl == 0) atomicMax(&bfar[r], __float_as_int(depth));
-      break;
-    }
-    float dd;
-    if (ds_at(s, dd) < thresh) {
-      if (ln.gl == 0) atomicMax(&bfar[r], __float_as_int(dd));
-      break;
-    }
-  }
-}
-
-static int coop_minb() {
-  static const int v = getenv("NMB_KNN_MINB") ? atoi(getenv("NMB_KNN_MINB")) : 8;
-  return v;
-}
-// launch helper: picks the instantiation for the tuned number of resident blocks per SM
-#define NMB_COOP_LAUNCH(kernel, nblocks, stream, ...)                                                      \
-  do {                                                                                                     \
-    const int mb_ = coop_minb();                                                                           \
-    if (mb_ >= 12) kernel<12><<<(unsigned)(nblocks), coop::BLOCK, 0, stream>>>(__VA_ARGS__);              \
-    else if (mb_ >= 10) kernel<10><<<(unsigned)(nblocks), coop::BLOCK, 0, stream>>>(__VA_ARGS__);         \
-    else if (mb_ >= 8) kernel<8><<<(unsigned)(nblocks), coop::BLOCK, 0, stream>>>(__VA_ARGS__);           \
-    else kernel<6><<<(unsigned)(nblocks), coop::BLOCK, 0, stream>>>(__VA_ARGS__);                         \
-  } while (0)
-
-// chains resident on the device at once (for sizing segments)
-static int64_t coop_resident_chains() { return (int64_t)sm_count() * coop_minb() * coop::GROUPS_PER_BLOCK; }
-constexpr int64_t COOP_RAY_KERNEL_MIN_RAYS = 2048;   // below this the per-point kernels expose more parallelism
 
 int launch_knn_lists(const nmb_grid* g, const float4* indicator_sorted, float w1, const float* xyz, const int32_t* off,
                      const int32_t* cnt, int64_t R, int64_t M, int max_list, KnnOut out, cudaStream_t stream) {
   if (M <= 0 || R <= 0) return 0;
   ProfScope prof(PROF_KNN_LIST, M, stream);
-  if (!knn_legacy()) {
-    // segments: enough chains for ~4 waves, at least 8 entries each
-    int64_t nseg = ceil_div(4 * coop_resident_chains(), R);
-    nseg = std::max<int64_t>(1, std::min<int64_t>(nseg, ceil_div(max_list, 8)));
-    const int seg = (int)ceil_div(max_list, nseg);
-    const int max_seg = (int)ceil_div(max_list, seg);
-    NMB_COOP_LAUNCH(knn_lists_coop_kernel, ceil_div(R * max_seg, coop::GROUPS_PER_BLOCK), stream, make_view(g),
-                    indicator_sorted, w1, xyz, off, cnt, R, seg, max_seg, out);
-    NMB_LAUNCH_OK();
-    return 0;
-  }
   // entries per thread: 16 when there is plenty of work (one cold walk per 16 queries); shorter segments when the lists
   // of a small shard (multi-GPU single-frame mode) would leave the GPU under-filled - only rays that hit the object have
   // entries at all, so the number of busy threads is ~M / seg, which should cover ~2 waves of the resident threads
@@ -838,8 +538,7 @@ int launch_knn_lists(const nmb_grid* g, const float4* indicator_sorted, float w1
   while (seg > 4 && M / seg < (int64_t)sm_count() * 1280 * 2) seg >>= 1;
   const int max_seg = (int)ceil_div(max_list, seg);
   knn_lists_kernel<<<(unsigned)ceil_div(R * max_seg, 128), 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1,
-                                                                            xyz, off, cnt, R, seg, max_seg, out,
-                                                                            make_view(g));
+                                                                            xyz, off, cnt, R, seg, max_seg, out);
   NMB_LAUNCH_OK();
   return 0;
 }
@@ -850,22 +549,6 @@ int launch_knn_distance(const nmb_grid* g, const float4* indicator_sorted, float
                         KnnOut out, cudaStream_t stream) {
   if (P <= 0) return 0;
   ProfScope prof(PROF_KNN, P, stream);
-  if (!knn_legacy()) {
-    if (!src.xyz && src.R >= COOP_RAY_KERNEL_MIN_RAYS && P % src.R == 0) {
-      const int S = (int)(P / src.R);
-      int64_t nseg = ceil_div(4 * coop_resident_chains(), src.R);
-      nseg = std::max<int64_t>(1, std::min<int64_t>(nseg, ceil_div(S, 8)));
-      const int seg = (int)ceil_div(S, nseg);
-      nseg = ceil_div(S, seg);
-      NMB_COOP_LAUNCH(knn_rays_coop_kernel, ceil_div(src.R * nseg, coop::GROUPS_PER_BLOCK), stream, make_view(g),
-                      indicator_sorted, w1, src, S, seg, out);
-    } else {
-      NMB_COOP_LAUNCH(knn_points_coop_kernel, ceil_div(P, coop::GROUPS_PER_BLOCK), stream, make_view(g),
-                      indicator_sorted, w1, src, P, out);
-    }
-    NMB_LAUNCH_OK();
-    return 0;
-  }
   if (!src.xyz && src.R >= RAY_KERNEL_MIN_RAYS && P % src.R == 0) {
     const int S = (int)(P / src.R);
     // segments per ray: enough threads for ~2 waves of the 1280 resident threads per SM (10 blocks of 128) - every segment
@@ -874,13 +557,8 @@ int launch_knn_distance(const nmb_grid* g, const float4* indicator_sorted, float
     nseg = std::max<int64_t>(1, std::min<int64_t>(nseg, ceil_div(S, 4)));   // at least 4 samples per segment
     const int seg = (int)ceil_div(S, nseg);
     nseg = ceil_div(S, seg);
-    static const int minb = getenv("NMB_KNN_MINB") ? atoi(getenv("NMB_KNN_MINB")) : 10;
-    const GridView gv = make_view(g);
-    static const int order = getenv("NMB_KNN_ORDER") ? atoi(getenv("NMB_KNN_ORDER")) : 1;   // 0 = full child sort (A/B)
-    const unsigned gridn = (unsigned)ceil_div(src.R * nseg, 128);
-    if (minb >= 12) { if (order) knn_rays_kernel<12, 1><<<gridn, 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1, src, S, seg, out, gv); else knn_rays_kernel<12, 0><<<gridn, 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1, src, S, seg, out, gv); }
-    else if (minb >= 10) { if (order) knn_rays_kernel<10, 1><<<gridn, 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1, src, S, seg, out, gv); else knn_rays_kernel<10, 0><<<gridn, 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1, src, S, seg, out, gv); }
-    else { if (order) knn_rays_kernel<8, 1><<<gridn, 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1, src, S, seg, out, gv); else knn_rays_kernel<8, 0><<<gridn, 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted, w1, src, S, seg, out, gv); }
+    knn_rays_kernel<<<(unsigned)ceil_div(src.R * nseg, 128), 128, 0, stream>>>(g->nodes.p, g->pts.p, indicator_sorted,
+                                                                               w1, src, S, seg, out);
     NMB_LAUNCH_OK();
     return 0;
   }
@@ -918,91 +596,12 @@ bound_scan_kernel(const float4* __restrict__ nodes, const float4* __restrict__ p
   }
 }
 
-// Ray-ordered bounded-near/far scan.  near = min, far = max over the samples with ds < thresh.  The n_grid samples of a
-// ray are split into segments of BOUND_SEG consecutive samples, one thread each (t = g * R + r): a thread walks its
-// segment from the front to its first hit (candidate for near, atomicMin on the depth bits) and from the back to its
-// last hit (candidate for far, atomicMax); samples between the two cannot change either extremum and are not
-// evaluated, and samples in cells of the shell certificate grid are decided without evaluation.  Output-identical to
-// evaluating all samples; the serial chain per thread is at most BOUND_SEG walks (short tails even with few rays).
-constexpr int BOUND_SEG = 32;
-
-__global__ void __launch_bounds__(128)
-bound_rays_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts,
-                  const float4* __restrict__ indicator, float w1, const float* __restrict__ rays_o,
-                  const float* __restrict__ dirs, const float* __restrict__ near, const float* __restrict__ far,
-                  int64_t R, int n_grid, float thresh, int32_t* __restrict__ bnear, int32_t* __restrict__ bfar,
-                  ShellGrid shell, const GridView gv) {
-  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  const int64_t r = t % R;
-  const int s_begin = (int)(t / R) * BOUND_SEG;
-  if (s_begin >= n_grid) return;
-  const int s_end = min(s_begin + BOUND_SEG, n_grid);
-  const float ox = rays_o[r * 3 + 0], oy = rays_o[r * 3 + 1], oz = rays_o[r * 3 + 2];
-  const float dx = dirs[r * 3 + 0], dy = dirs[r * 3 + 1], dz = dirs[r * 3 + 2];
-  const float nr = near[r], fr = far[r];
-  float d2[KNN_K];
-  int32_t ix[KNN_K];
-  bool have_prev = false;   // d2 / ix hold the neighbours of some earlier sample of this ray (valid warm start)
-  // returns the mesh distance at sample s, or +inf / -inf when the sample lies in a cell certified to be outside /
-  // inside the shell
-  auto ds_at = [&](int s, float& depth) {
-    const float tt = linspace01(s, n_grid);
-    depth = __fadd_rn(__fmul_rn(nr, __fsub_rn(1.0f, tt)), __fmul_rn(fr, tt));  // renderer.py:81
-    const float qx = __fadd_rn(ox, __fmul_rn(depth, dx));
-    const float qy = __fadd_rn(oy, __fmul_rn(depth, dy));
-    const float qz = __fadd_rn(oz, __fmul_rn(depth, dz));
-    if (shell.cells) {
-      const float sc = 0.5f * (float)shell.G / shell.B;
-      const float fx = (qx + shell.B) * sc, fy = (qy + shell.B) * sc, fz = (qz + shell.B) * sc;
-      if (fx >= 0.f && fy >= 0.f && fz >= 0.f && fx < (float)shell.G && fy < (float)shell.G && fz < (float)shell.G) {
-        const int64_t cell = ((int64_t)(int)fz * shell.G + (int)fy) * shell.G + (int)fx;
-        const uint8_t code = __ldg(shell.cells + cell);
-        if (code == 1) return CUDART_INF_F;    // proven outside the shell: mask false
-        if (code == 2) return -CUDART_INF_F;   // proven inside the shell: mask true (only the depth matters)
-      } else {
-        const float ex = qx - shell.cx, ey = qy - shell.cy, ez = qz - shell.cz;
-        if (ex * ex + ey * ey + ez * ez >= shell.far_r * shell.far_r) return CUDART_INF_F;
-      }
-    }
-    const bool warm = have_prev;
-    have_prev = true;
-    if (warm) {
-      warm_rerank<KNN_K>(pts, qx, qy, qz, d2, ix);
-      knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix, NMB_GV_ARG(gv));
-    } else {
-      knn_walk<KNN_K, false>(nodes, pts, qx, qy, qz, d2, ix);
-    }
-    float w[KNN_K], ds, grad[3];
-    mesh_distance_point(pts, indicator, w1, qx, qy, qz, d2, ix, w, ds, grad);
-    return ds;
-  };
-  int first = -1;
-  float depth = 0.f;
-  for (int s = s_begin; s < s_end; ++s) {
-    if (ds_at(s, depth) < thresh) {
-      first = s;
-      atomicMin(&bnear[r], __float_as_int(depth));   // depths are >= 0: their bit patterns order like the values
-      break;
-    }
-  }
-  if (first < 0) return;  // no hit in this segment
-  for (int s = s_end - 1; s >= first; --s) {
-    // s == first is known to be a hit: the loop always terminates with a far candidate
-    if (s == first) {
-      atomicMax(&bfar[r], __float_as_int(depth));   // `depth` still holds sample `first` unless overwritten below
-      break;
-    }
-    float dd;
-    if (ds_at(s, dd) < thresh) {
-      atomicMax(&bfar[r], __float_as_int(dd));
-      break;
-    }
-  }
-}
-
-// Two-ended variant of the ray-ordered scan (the default for frame-sized batches): only the FIRST and the LAST hit of
-// a ray matter, so the front-to-back search and the back-to-front search are separate launches that talk to each other
-// through bnear / bfar:
+// Ray-ordered bounded near / far for frame-sized batches: near = min, far = max over the samples with ds < thresh.  The
+// n_grid samples of a ray are split into segments of BOUND_SEG consecutive samples, one thread each (t = g * R + r), and
+// samples in cells of the shell certificate grid are decided without evaluation.  Output-identical to evaluating all
+// samples; the serial chain per thread is at most BOUND_SEG walks (short tails even with few rays).
+// Only the FIRST and the LAST hit of a ray matter, so the front-to-back search and the back-to-front search are separate
+// launches that talk to each other through bnear / bfar:
 //   launch 1 (BACKWARD = false): thread (segment g ascending, ray r) looks for the first hit of its segment, but gives
 //     up as soon as bnear[r] shows a hit in front of the sample it is about to evaluate;
 //   launch 2 (BACKWARD = true):  thread (segment g DESCENDING, ray r) looks for the last hit of its segment between the
@@ -1011,14 +610,15 @@ bound_rays_kernel(const float4* __restrict__ nodes, const float4* __restrict__ p
 // finished; a stale read only costs work, never correctness (bnear / bfar only move towards their final values, and a
 // thread only skips samples that provably cannot change them).  Rays that cross the object evaluate the two OUTER
 // crossings of the 0.1 shell only - not the inner boundary of the shell (ds rises above 0.1 again deep inside the
-// object) - and rays without any hit are scanned once, not twice.  Depths are taken to be non-decreasing along a ray,
-// as in bound_rays_kernel.
+// object) - and rays without any hit are scanned once, not twice.  Depths are taken to be non-decreasing along a ray.
+constexpr int BOUND_SEG = 32;
+
 template <bool BACKWARD>
 __global__ void __launch_bounds__(128)
 bound_dir_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pts, const float4* __restrict__ indicator,
                  float w1, const float* __restrict__ rays_o, const float* __restrict__ dirs,
                  const float* __restrict__ near, const float* __restrict__ far, int64_t R, int n_grid, float thresh,
-                 int32_t* __restrict__ bnear, int32_t* __restrict__ bfar, ShellGrid shell, const GridView gv) {
+                 int32_t* __restrict__ bnear, int32_t* __restrict__ bfar, ShellGrid shell) {
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t r = t % R;
   const int nseg = (n_grid + BOUND_SEG - 1) / BOUND_SEG;
@@ -1075,7 +675,7 @@ bound_dir_kernel(const float4* __restrict__ nodes, const float4* __restrict__ pt
       if (BACKWARD ? (__ldcg(bfar + r) >= dbits) : (__ldcg(bnear + r) < dbits)) return;
       if (have_prev) {
         warm_rerank<KNN_K>(pts, qx, qy, qz, d2, ix);
-        knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix, NMB_GV_ARG(gv));
+        knn_walk<KNN_K, true>(nodes, pts, qx, qy, qz, d2, ix);
       } else {
         knn_walk<KNN_K, false>(nodes, pts, qx, qy, qz, d2, ix);
         have_prev = true;
@@ -1098,35 +698,14 @@ int launch_bound_scan(const nmb_grid* g, const float4* indicator, float w1, cons
   const int64_t n = R * n_grid;
   if (n <= 0) return 0;
   ProfScope prof(PROF_BOUND, n, stream);
-  if (!knn_legacy()) {
-    if (R >= COOP_RAY_KERNEL_MIN_RAYS) {
-      const int64_t nseg = ceil_div(n_grid, BOUND_SEG_COOP);
-      NMB_COOP_LAUNCH(bound_rays_coop_kernel, ceil_div(R * nseg, coop::GROUPS_PER_BLOCK), stream, make_view(g), indicator,
-                      w1, rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar, (thresh == 0.1f) ? shell : ShellGrid{});
-    } else {
-      NMB_COOP_LAUNCH(bound_scan_coop_kernel, ceil_div(n, coop::GROUPS_PER_BLOCK), stream, make_view(g), indicator, w1,
-                      rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar);
-    }
-    NMB_LAUNCH_OK();
-    return 0;
-  }
-  static const bool two_ended = getenv("NMB_BOUND_ONE_PASS") == nullptr;
-  if (R >= RAY_KERNEL_MIN_RAYS && two_ended) {
+  if (R >= RAY_KERNEL_MIN_RAYS) {
     const int64_t nseg = ceil_div(n_grid, BOUND_SEG);
     const ShellGrid sg = (thresh == 0.1f) ? shell : ShellGrid{};
     bound_dir_kernel<false><<<(unsigned)ceil_div(R * nseg, 128), 128, 0, stream>>>(
-        g->nodes.p, g->pts.p, indicator, w1, rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar, sg, make_view(g));
+        g->nodes.p, g->pts.p, indicator, w1, rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar, sg);
     NMB_LAUNCH_OK();
     bound_dir_kernel<true><<<(unsigned)ceil_div(R * nseg, 128), 128, 0, stream>>>(
-        g->nodes.p, g->pts.p, indicator, w1, rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar, sg, make_view(g));
-    NMB_LAUNCH_OK();
-    return 0;
-  }
-  if (R >= RAY_KERNEL_MIN_RAYS) {
-    const int64_t nseg = ceil_div(n_grid, BOUND_SEG);
-    bound_rays_kernel<<<(unsigned)ceil_div(R * nseg, 128), 128, 0, stream>>>(
-        g->nodes.p, g->pts.p, indicator, w1, rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar,
-        (thresh == 0.1f) ? shell : ShellGrid{}, make_view(g));
+        g->nodes.p, g->pts.p, indicator, w1, rays_o, dirs, near, far, R, n_grid, thresh, bnear, bfar, sg);
     NMB_LAUNCH_OK();
     return 0;
   }

@@ -14,11 +14,6 @@ struct nmb_grid {
   nmb::DevBuf<int32_t> order;  // [V] sorted slot -> original index
   nmb::DevBuf<int32_t> inv;    // [V] original index -> sorted slot
   nmb::DevBuf<float4> nodes;   // [NODE_F4*num_nodes]: box + disc bounds and child / point links; see grid.cu
-  // directory start of the cooperative walk (knn_coop.cuh): per level l in [dir_lmin, dir_lmax] a dense table of 8^l
-  // entries indexed by the Morton prefix: octree node id with that prefix, its leaf ancestor, or -1 (empty cell)
-  nmb::DevBuf<int32_t> dir;
-  int dir_lmin = 0, dir_lmax = -1;
-  int32_t dir_off[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   std::vector<int32_t> lvl_off; // first node id of every octree level (+ end sentinel); children ids > parent ids
 };
 
@@ -29,17 +24,6 @@ constexpr int LEAF_MAX = 32;      // nodes with <= LEAF_MAX points are leaves (m
 constexpr int NODE_F4 = 4;        // float4 per node: {lo, link}, {hi, count}, {centre, r}, {axis, t}
 constexpr int DISC_MAX_POINTS = 8192;  // nodes larger than this get the trivial disc (sphere) bound
 constexpr int STACK_MAX = 96;     // traversal stack entries (7 * depth + 8 <= 78 for depth 10)
-
-// device view of the index (passed by value in kernel parameters)
-struct GridView {
-  const float4* nodes;
-  const float4* pts;
-  const int32_t* dir;       // directory tables, levels dir_lmin.. back to back (8^l entries each); nullptr = none
-  int dir_lmin, dir_lmax;   // directory levels (inclusive); dir_lmax < dir_lmin = none
-  float bmin[3];
-  float inv_cell;           // 2^levels / cube side
-  int levels;
-};
 
 // Per-point outputs of the fused KNN + mesh-distance kernel, structure-of-arrays with stride `stride`
 // (element (k, p) at [k * stride + p]) so that a warp of consecutive points reads/writes coalesced.

@@ -43,15 +43,7 @@ __device__ __forceinline__ float disc_bound(float qx, float qy, float qz, const 
 
 __device__ __forceinline__ float node_bound(float qx, float qy, float qz, const float4& lo, const float4& hi,
                                             const float4& cr, const float4& ut) {
-  const float bd = box_dist_rn(qx, qy, qz, lo, hi);
-  const float dx = qx - cr.x, dy = qy - cr.y, dz = qz - cr.z;
-  const float a = ut.x * dx + ut.y * dy + ut.z * dz;
-  const float dd = dx * dx + dy * dy + dz * dz;
-  const float b = sqrtf(fmaxf(dd - a * a, 0.f));
-  const float h = fmaxf(fabsf(a) - ut.w, 0.f);
-  const float l = fmaxf(b - cr.w, 0.f);
-  const float disc = (h * h + l * l) * 0.99998f - 1e-12f;
-  return fmaxf(bd, disc);
+  return fmaxf(box_dist_rn(qx, qy, qz, lo, hi), disc_bound(qx, qy, qz, cr, ut));
 }
 
 // Candidates are ranked by the total order (squared distance, slot index): the K smallest under it are unique, so
@@ -105,91 +97,9 @@ __device__ __forceinline__ void topk_insert(float (&d)[K], int32_t (&ix)[K], flo
 //   WARM = true : the caller pre-loaded d[] / ix[] with K DISTINCT real points and their distances to q, sorted
 //                 ascending (e.g. the neighbours of the previous sample on the same ray).  The walk then starts with
 //                 a tight pruning bound; a point already in the list is never inserted twice.
-__device__ __forceinline__ uint32_t spread_bits10(uint32_t v) {
-  v = (v * 0x00010001u) & 0xFF0000FFu;
-  v = (v * 0x00000101u) & 0x0F00F00Fu;
-  v = (v * 0x00000011u) & 0xC30C30C3u;
-  v = (v * 0x00000005u) & 0x49249249u;
-  return v;
-}
-
-// Directory start of a WARM walk (see the header of knn_coop.cuh for the construction and the exactness argument): the
-// ball (q, sqrt(worst)) contains every candidate that could still enter the list; the finest directory level whose
-// cells are at least as wide as the ball's extent maps it to at most 2 x 2 x 2 cells, whose nodes replace the root as
-// the initial stack.  Returns the number of entries pushed (possibly 0: nothing can improve the list), or -1 when no
-// directory level fits (the caller starts from the root).
-__device__ __forceinline__ int dir_seed(const GridView& gv, float qx, float qy, float qz, float worst, int32_t* sn,
-                                        float* sd) {
-  const float r = sqrtf(worst) * 1.00001f + 1e-6f;
-  const int maxc = (1 << gv.levels) - 1;
-  const float q[3] = {qx, qy, qz};
-  int lo[3], hi[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const float tl = (__fsub_rn(q[c], r) - gv.bmin[c]) * gv.inv_cell;
-    const float th = (__fadd_rn(q[c], r) - gv.bmin[c]) * gv.inv_cell;
-    lo[c] = min(max((int)floorf(fmaxf(tl, -1.f)), 0), maxc);
-    hi[c] = min(max((int)floorf(fminf(th, 1.0e9f)), 0), maxc);
-  }
-  int lev = -1;
-  for (int l = gv.dir_lmax; l >= gv.dir_lmin; --l) {
-    const int sh = gv.levels - l;
-    if ((hi[0] >> sh) - (lo[0] >> sh) <= 1 && (hi[1] >> sh) - (lo[1] >> sh) <= 1 && (hi[2] >> sh) - (lo[2] >> sh) <= 1) {
-      lev = l;
-      break;
-    }
-  }
-  if (lev < 0) return -1;
-  const int sh = gv.levels - lev;
-  const int bx = lo[0] >> sh, by = lo[1] >> sh, bz = lo[2] >> sh;
-  const int nx = (hi[0] >> sh) - bx, ny = (hi[1] >> sh) - by, nz = (hi[2] >> sh) - bz;
-  const int32_t* tab = gv.dir + (int32_t)(((1u << (3 * lev)) - (1u << (3 * gv.dir_lmin))) / 7u);
-  float cd[8];
-  int32_t cn[8];
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    cd[c] = CUDART_INF_F;
-    cn[c] = -1;
-    const int dx = c & 1, dy = (c >> 1) & 1, dz = c >> 2;
-    if (dx <= nx && dy <= ny && dz <= nz) {
-      const uint32_t m = (spread_bits10((uint32_t)(bx + dx)) << 2) | (spread_bits10((uint32_t)(by + dy)) << 1) |
-                         spread_bits10((uint32_t)(bz + dz));
-      const int32_t nid = __ldg(tab + m);
-      bool dup = false;   // several cells may map to one leaf ancestor: keep its first occurrence only
-#pragma unroll
-      for (int e = 0; e < c; ++e) dup |= (cn[e] == nid);
-      cn[c] = nid;
-      if (nid >= 0 && !dup) {
-        const float4* nc = gv.nodes + NODE_F4 * (int64_t)nid;
-        float bd = box_dist_rn(qx, qy, qz, __ldg(nc), __ldg(nc + 1));
-        if (bd <= worst) {
-          bd = fmaxf(bd, disc_bound(qx, qy, qz, __ldg(nc + 2), __ldg(nc + 3)));
-          if (bd <= worst) cd[c] = bd;
-        }
-      }
-    }
-  }
-  NMB_SORT8_DESC()   // nearest cell ends up pushed last
-  int sp = 0;
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    if (cd[c] < CUDART_INF_F) {
-      sn[sp] = cn[c];
-      sd[sp] = cd[c];
-      ++sp;
-    }
-  }
-  return sp;
-}
-
-// ORDER = 0: surviving children are pushed fully sorted (farthest first); ORDER = 1 (default): only the
-// NEAREST survivor is put on top of the stack, the others keep child order (7 compare / selects instead of the
-// 19-comparator network; any push order is exact - the pop test prunes - only the pruning efficiency can differ).
-// Both orders give bit-identical results (tools/knn_ab.py compares them).
-template <int K, bool WARM, int ORDER = 1>
+template <int K, bool WARM>
 __device__ __forceinline__ void knn_walk(const float4* __restrict__ nodes, const float4* __restrict__ pts, float qx,
-                                         float qy, float qz, float (&d)[K], int32_t (&ix)[K],
-                                         const GridView* gv = nullptr) {
+                                         float qy, float qz, float (&d)[K], int32_t (&ix)[K]) {
   if (!WARM) {
 #pragma unroll
     for (int k = 0; k < K; ++k) {
@@ -199,13 +109,9 @@ __device__ __forceinline__ void knn_walk(const float4* __restrict__ nodes, const
   }
   int32_t sn[STACK_MAX];
   float sd[STACK_MAX];
-  int sp = -1;
-  if (WARM && gv != nullptr && gv->dir != nullptr) sp = dir_seed(*gv, qx, qy, qz, d[K - 1], sn, sd);
-  if (sp < 0) {
-    sp = 1;
-    sn[0] = 0;
-    sd[0] = 0.f;
-  }
+  int sp = 1;
+  sn[0] = 0;
+  sd[0] = 0.f;
   // "while-while" traversal: every lane first descends through INTERNAL nodes until it holds a leaf, then all lanes
   // of the warp scan their leaves together - the two code paths are not interleaved lane by lane, which keeps far
   // more lanes active per issued instruction than a single pop-and-branch loop.
@@ -256,37 +162,27 @@ __device__ __forceinline__ void knn_walk(const float4* __restrict__ nodes, const
         sd[sp] = cd[only];
         ++sp;
       } else if (m > 1) {
-        if (ORDER == 0) {
-          NMB_SORT8_DESC()   // nearest child ends up pushed last
+        // only the nearest survivor goes on top of the stack, the others keep child order: any push order is exact
+        // (the pop test prunes), only the pruning efficiency depends on it
+        float best = cd[0];
+        int bi = 0;
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            if (cd[c] < CUDART_INF_F) {
-              sn[sp] = cn[c];
-              sd[sp] = cd[c];
-              ++sp;
-            }
-          }
-        } else {
-          float best = cd[0];
-          int bi = 0;
-#pragma unroll
-          for (int c = 1; c < 8; ++c) {
-            const bool lt = cd[c] < best;
-            best = lt ? cd[c] : best;
-            bi = lt ? c : bi;
-          }
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            if (cd[c] < CUDART_INF_F && c != bi) {
-              sn[sp] = cn[c];
-              sd[sp] = cd[c];
-              ++sp;
-            }
-          }
-          sn[sp] = link + bi;
-          sd[sp] = best;
-          ++sp;
+        for (int c = 1; c < 8; ++c) {
+          const bool lt = cd[c] < best;
+          best = lt ? cd[c] : best;
+          bi = lt ? c : bi;
         }
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          if (cd[c] < CUDART_INF_F && c != bi) {
+            sn[sp] = cn[c];
+            sd[sp] = cd[c];
+            ++sp;
+          }
+        }
+        sn[sp] = link + bi;
+        sd[sp] = best;
+        ++sp;
       }
     }
     if (leaf_e == leaf_b) break;   // stack exhausted without another leaf
@@ -326,6 +222,5 @@ __device__ __forceinline__ void warm_rerank(const float4* __restrict__ pts, floa
   }
 }
 #undef NMB_CSWAP
-
 
 }  // namespace nmb

@@ -17,16 +17,14 @@
 // point by point; the first vertex that cannot be bounded above the threshold makes the cell "uncertain".
 #include <math_constants.h>
 
-#include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
 #include "field.cuh"
 #include "knn_walk.cuh"
 
 namespace nmb {
 
-constexpr int SHELL_G_DEFAULT = 128;   // cells per axis (NMB_SHELL_G overrides, for experiments)
+constexpr int SHELL_G = 128;               // cells per axis
 constexpr float SHELL_B = 1.001f;          // grid covers [-B, B]^3 (the unit bounding sphere of the reference's scenes)
 constexpr float SHELL_THR = 0.1f + 2e-3f;  // certificate threshold: renderer.py:73 distance_thresh + rounding margin
 constexpr float SHELL_THR_IN = 0.1f - 2e-3f;  // "inside" certificate: every point of the cell has ds < 0.1
@@ -185,8 +183,6 @@ int ensure_shell_grid(const nmb_field* f, cudaStream_t stream) {
   f->shell = ShellGrid{};
   f->shell_valid = true;   // whatever happens below, do not retry on every frame
   if (g->lvl_off.size() < 2 || !(f->w1 > 0.f)) return 0;
-  int SHELL_G = SHELL_G_DEFAULT;
-  if (const char* e = getenv("NMB_SHELL_G")) SHELL_G = std::max(16, std::min(512, atoi(e)));
   NMB_CUDA_OK(f->node_normals.alloc(g->num_nodes));
   NMB_CUDA_OK(f->shell_cells.alloc((int64_t)SHELL_G * SHELL_G * SHELL_G));
   for (int l = (int)g->lvl_off.size() - 2; l >= 0; --l) {
