@@ -139,6 +139,8 @@ static int pack_field(const nmb_field_desc* d, nmb_field* f, cudaStream_t stream
             "unsupported MLP depth");
   NMB_CHECK(d->multires_d >= 0 && d->multires_fg >= 0 && d->multires_ft >= 0 && d->multires_view >= 0,
             "identity embedders (multires < 0) are not supported by the fused kernels");
+  NMB_CHECK(f->engine != 2 || d->multires_d <= F16_MAX_MULTIRES_D,
+            "multires_d > 16 overflows the fp16 engine's tangent operands (use the 3xTF32 engine)");
   f->lay = make_layout(d);
   f->shell_valid = false;
   f->shell = ShellGrid{};

@@ -8,6 +8,9 @@ namespace nmb {
 constexpr int MLP_W = 256;     // hidden width the fused kernels are specialised for
 constexpr int FEAT = 32;       // feature block: vertex codes are processed 32 columns at a time (code width = 32 n)
 constexpr int MAX_LAYERS = 8;
+// fp16 engine: the tangent seed of PE(ds) band b is 2^b cos(2^b ds), an fp16 A operand, so the highest band
+// (2^(multires_d - 1)) must stay below fp16's largest finite value 65504
+constexpr int F16_MAX_MULTIRES_D = 16;
 
 // Column layout of the first-layer inputs (our own order; weights are permuted to match at pack time).
 //   geometry: [PE(ds) | 0-pad to 16 | fg, sin fg, cos fg, sin 2fg, cos 2fg, ...]            K0g (multiple of 16)

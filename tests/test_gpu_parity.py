@@ -644,8 +644,9 @@ def test_detailed_and_samples_output_shapes(case5):
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dims", [(64, 96), (256, 256)])
 def test_config3_wide_vertex_codes_vs_oracle(dims):
-    """"8-NN 256-d vertex codes" (BASELINE.json configs[2]): the tcgen05 engine walks the first layer in 32-column code
-    blocks (geometry input 17 + 5 * 256 = 1297 columns), checked against the oracle point-wise and through a render."""
+    """"8-NN 256-d vertex codes" (BASELINE.json configs[2]): both tensor-core engines walk the first layer in 32-column
+    code blocks (geometry input 17 + 5 * 256 = 1297 columns), checked against the oracle point-wise and through a
+    render."""
     import neumesh_b200 as nb
     from oracle import render as orender
     dev = _dev()
@@ -653,39 +654,41 @@ def test_config3_wide_vertex_codes_vs_oracle(dims):
     mesh = synth.icosphere_mesh(5, seed=0)
     sd = synth.make_state_dict(mesh, cfg, seed=1)
     f = helpers.oracle_field(mesh, cfg, sd)
-    model = helpers.cuda_model(mesh, cfg, sd, "tcgen05")
-    assert model.fused_supported()
     x, v = helpers.sample_points(3001, seed=22)
-    with torch.no_grad():
-        sdf = model.forward_density_only(x.to(dev))
-        sdf_n, nabla = model.forward_with_nablas(x.to(dev))
-        sdf_c, rgb = model.forward(x.to(dev), v.to(dev))
     s_ref = f.forward_density_only(x)
     _, n_ref = f.forward_with_nablas(x)
     _, c_ref = f.forward(x, v)
-    e_sdf = (sdf.cpu() - s_ref).abs().max().item()
-    e_nab = (nabla.cpu() - n_ref).abs().max().item()
-    e_rgb = (rgb.cpu() - c_ref).abs().max().item()
-    print(f"codes {dims}: max-abs vs oracle: sdf {e_sdf:.3e} nabla {e_nab:.3e} rgb {e_rgb:.3e}")
-    assert e_sdf < 1e-5 and e_nab < 1e-4 and e_rgb < 1e-5
-    assert torch.equal(sdf, sdf_c) and torch.equal(sdf, sdf_n)
+    o, d = synth.frame_rays(20, 20, view=2)
+    kw = dict(calc_normal=True, white_bkgd=True, bounded_near_far=True)
+    r_ref, d_ref, _ = orender.volume_render(o, d, f, detailed_output=False, **kw)
+    for engine in ("tcgen05", "tcgen05_f16"):
+        model = helpers.cuda_model(mesh, cfg, sd, engine)
+        assert model.fused_supported()
+        with torch.no_grad():
+            sdf = model.forward_density_only(x.to(dev))
+            sdf_n, nabla = model.forward_with_nablas(x.to(dev))
+            sdf_c, rgb = model.forward(x.to(dev), v.to(dev))
+        e_sdf = (sdf.cpu() - s_ref).abs().max().item()
+        e_nab = (nabla.cpu() - n_ref).abs().max().item()
+        e_rgb = (rgb.cpu() - c_ref).abs().max().item()
+        print(f"[{engine}] codes {dims}: max-abs vs oracle: sdf {e_sdf:.3e} nabla {e_nab:.3e} rgb {e_rgb:.3e}")
+        assert e_sdf < 1e-5 and e_nab < 1e-4 and e_rgb < 1e-5
+        assert torch.equal(sdf, sdf_c) and torch.equal(sdf, sdf_n)
+        # render: free-running against the oracle on a small frame
+        with torch.no_grad():
+            r, dep, ex = nb.volume_render(o.to(dev), d.to(dev), model, detailed_output=False, **kw)
+        dr = (r.cpu() - r_ref).abs().max(-1)[0]
+        dd = (dep.cpu() - d_ref).abs()
+        ok = ((dr <= RGB_TOL) & (dd <= DEPTH_TOL)).float().mean().item()
+        print(f"[{engine}] codes {dims}: rays within (1e-4, 1e-5) of the oracle render: {ok:.3f}; median rgb "
+              f"{dr.median():.1e} depth {dd.median():.1e}")
+        assert 1.0 - ok <= outlier_bound(REF_FLOOR["config3"], dr.numel()) and dr.median() <= 1e-6 and dd.median() <= 1e-6
+        del model
     # the fp32 engine has no wide-code path and must say so instead of computing something else
     m32 = helpers.cuda_model(mesh, cfg, sd, "fp32")
     assert not m32.fused_supported()
     with pytest.raises(RuntimeError):
         m32.packed_field()
-    # render: free-running against the oracle on a small frame
-    o, d = synth.frame_rays(20, 20, view=2)
-    kw = dict(calc_normal=True, white_bkgd=True, bounded_near_far=True)
-    with torch.no_grad():
-        r, dep, ex = nb.volume_render(o.to(dev), d.to(dev), model, detailed_output=False, **kw)
-    r_ref, d_ref, _ = orender.volume_render(o, d, f, detailed_output=False, **kw)
-    dr = (r.cpu() - r_ref).abs().max(-1)[0]
-    dd = (dep.cpu() - d_ref).abs()
-    ok = ((dr <= RGB_TOL) & (dd <= DEPTH_TOL)).float().mean().item()
-    print(f"codes {dims}: rays within (1e-4, 1e-5) of the oracle render: {ok:.3f}; median rgb {dr.median():.1e} "
-          f"depth {dd.median():.1e}")
-    assert 1.0 - ok <= outlier_bound(REF_FLOOR["config3"], dr.numel()) and dr.median() <= 1e-6 and dd.median() <= 1e-6
 
 
 def test_config5_large_mesh_256_samples_per_ray():

@@ -73,7 +73,7 @@ def test_texture_dropin_torch_path_cpu(golden_dir):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("engine", ["tcgen05", "fp32"])
+@pytest.mark.parametrize("engine", ["tcgen05", "fp32", "tcgen05_f16"])
 def test_texture_dropin_fused_vs_oracle_and_golden(golden_dir, engine):
     import neumesh_b200 as nb
     from neumesh_b200 import _lib

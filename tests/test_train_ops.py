@@ -138,7 +138,19 @@ def test_tr_gemm_vs_torch():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("cfg_kw", [dict(), dict(enable_nablas_input=False, geometry_dim=64, color_dim=96)])
+@pytest.mark.parametrize("cfg_kw", [
+    dict(), dict(enable_nablas_input=False, geometry_dim=64, color_dim=96),
+    # rows B, C, E of tests/test_field_envelope.py: one hidden geometry layer and raw codes only; the deepest geometry
+    # net with 64-d colour codes (multires_d 8 instead of 16: the kernels and the float64 torch sequence compute ds
+    # independently, and a 2^15 band turns their fp32 / float64 difference in ds into a 1e-3 one in the encoding);
+    # one colour layer with 96-d / 160-d codes and 6 view bands
+    dict(D_density=1, D_color=4, multires_d=4, multires_fg=0, multires_ft=2, multires_view=4,
+         learn_indicator_weight=True),
+    dict(D_density=7, D_color=2, color_dim=64, multires_d=8, multires_fg=3, multires_ft=1, multires_view=2,
+         learn_indicator_weight=True),
+    dict(D_density=2, D_color=1, geometry_dim=96, color_dim=160, multires_d=8, multires_fg=1, multires_ft=0,
+         multires_view=6, learn_indicator_weight=True),
+])
 def test_tr_kernels_and_field_op_vs_torch_primitives(cfg_kw):
     """field_forward / field_backward on the CUDA kernels vs the same sequencing on torch primitives (same device, in
     float64, so that the reference's own rounding cannot decide the result): every intermediate the kernels produce is
