@@ -173,6 +173,39 @@ int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_
                int64_t rays_per_chunk, float* rgb, float* depth, float* acc, float* normals,
                const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- texture edit --------------------------------------------------------------------------------------------
+ * TextureEditableNeuMesh (editing/texture_neumesh/texture_neumesh.py:8-122), rendered by
+ * editing/texture_neumesh/texture_renderer.py:63-75 through render.py:render_function.  Geometry is the main model's;
+ * for every colour point, with the main mesh's neighbours idx / weights w and for each reference model i in order
+ * (texture_neumesh.py:81-121): m_k = masks[i][idx_k]; w_paint = sum w_k m_k, w_rest = sum w_k (1 - m_k); where
+ * w_paint > 0 the main colour c becomes c * w_rest / (w_paint + w_rest) + c_ref * w_paint / (w_paint + w_rest), c_ref
+ * being reference i's colour network on ds, R_i view_dir, R_i nabla, the edited code table, idx and the weights
+ * w_k m_k / (w_paint + 1e-8).  Only the reference fields' colour networks are used (their grids are never walked);
+ * they may differ from the main field in colour configuration and MLP engine.
+ *   masks      device uint8 [n_ref, V] (non-zero = painted), V = vertices of the main field's mesh, original order
+ *   codes      device fp32 [V, color_dim] (main_editing_colorfeats), original order; color_dim = every reference
+ *              field's color_dim
+ *   rotations  HOST fp32 [n_ref, 9] row-major main -> reference rotations (rot_s_m), or NULL for none
+ * Create / update copy (and permute to the main grid's slot order) what they are given and synchronise the stream.
+ * The edit refers to the fields it was created with: they must outlive it; re-packing them in place
+ * (nmb_field_update) is fine. */
+typedef struct nmb_edit nmb_edit;
+int nmb_edit_create(const nmb_field* main_field, int32_t n_ref, const nmb_field* const* ref_fields,
+                    const uint8_t* masks, const float* codes, int64_t V, int32_t color_dim,
+                    const float* rotations_host, void* stream, nmb_edit** out);
+/* new values for masks, codes and rotations (same shapes as at creation) */
+int nmb_edit_update(nmb_edit* e, const uint8_t* masks, const float* codes, const float* rotations_host, void* stream);
+void nmb_edit_destroy(nmb_edit* e);
+/* bytes of scratch nmb_render_edit needs for `rays_per_chunk` rays (== nmb_render_workspace_bytes when edit is NULL) */
+int64_t nmb_render_edit_workspace_bytes(const nmb_render_cfg* cfg, const nmb_edit* edit, int64_t rays_per_chunk);
+/* nmb_render of the edited model (texture_renderer.py:63-75 -> renderer.py:105-368): the main field `f` (the one the
+ * edit was created with) drives the sampling cascade, sdf, weights, normals and depth; the colour of every evaluated
+ * mid-point is blended as above (detail->radiance holds the blended colour).  sampling_only is not accepted. */
+int nmb_render_edit(const nmb_field* f, const nmb_edit* edit, const nmb_render_cfg* cfg, const float* rays_o,
+                    const float* rays_d, int64_t N, int64_t rays_per_chunk, float* rgb, float* depth, float* acc,
+                    float* normals, const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes,
+                    void* stream);
+
 /* One hierarchical up-sampling step (renderer.py:209-245 + utils/rend_util.py:276-319 sample_pdf, det=True):
  * from n sorted depths z and their sdf values, the n_new inverse-CDF depths for sharpness inv_s (= 256 * 2^iter).
  * SAMPLE-MAJOR arrays: z, sdf [n, N]; z_new [n_new, N]; scratch [n, N]. */

@@ -69,6 +69,12 @@ SIGNATURES = {
     "nmb_render_workspace_bytes": (_I64, [C.POINTER(RenderCfg), _I64]),
     "nmb_render": (C.c_int, [_P, C.POINTER(RenderCfg), _P, _P, _I64, _I64, _P, _P, _P, _P, C.POINTER(RenderDetail),
                              _P, _I64, _P]),
+    "nmb_edit_create": (C.c_int, [_P, _I32, C.POINTER(_P), _P, _P, _I64, _I32, C.POINTER(_F), _P, C.POINTER(_P)]),
+    "nmb_edit_update": (C.c_int, [_P, _P, _P, C.POINTER(_F), _P]),
+    "nmb_edit_destroy": (None, [_P]),
+    "nmb_render_edit_workspace_bytes": (_I64, [C.POINTER(RenderCfg), _P, _I64]),
+    "nmb_render_edit": (C.c_int, [_P, _P, C.POINTER(RenderCfg), _P, _P, _I64, _I64, _P, _P, _P, _P,
+                                  C.POINTER(RenderDetail), _P, _I64, _P]),
     "nmb_upsample_step": (C.c_int, [_P, _P, _I64, _I32, _I32, _F, _P, _P, _P]),
     "nmb_first_crossing": (C.c_int, [_P, _I64, _I32, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "nmb_pack_bgr8": (C.c_int, [_P, _I64, _P, _P]),

@@ -79,6 +79,51 @@ struct DeviceOnce {
   }
 };
 
+// torch.sum over a contiguous fp32 row of n elements as ATen's CPU kernel computes it (SumKernel.cpp, the path
+// `weights.sum(dim=-1)` of rend_util.py:281 takes; checked against torch 2.11 for every n <= 255, AVX2 and AVX512
+// builds alike): the row is read as 8-lane vectors; four vector accumulators take vectors 4i, 4i+1, 4i+2, 4i+3, leftover
+// vectors go to accumulator 0, the accumulators are folded 0 += 1, 2, 3; then a scalar starts from 0, adds the tail
+// elements (n % 8) in order and finally the 8 lanes in order.  Rows shorter than 8 use four scalar accumulators in the
+// same pattern.  sample_pdf's u = 1 sample (searchsorted against a cdf that saturates at 1.0 or not) depends on these
+// bits, so the normalisation constant is reproduced exactly rather than summed sequentially.
+__device__ __forceinline__ float torch_row_sum(const float* __restrict__ x, int64_t stride, int n) {
+  if (n < 8) {
+    float a[4] = {0.f, 0.f, 0.f, 0.f};
+    const int q = n / 4;
+    if (q) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) a[k] = __fadd_rn(a[k], x[k * stride]);
+    }
+    for (int i = q * 4; i < n; ++i) a[0] = __fadd_rn(x[i * stride], a[0]);
+    a[0] = __fadd_rn(a[0], a[1]);
+    a[0] = __fadd_rn(a[0], a[2]);
+    return __fadd_rn(a[0], a[3]);
+  }
+  float acc[4][8];
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int l = 0; l < 8; ++l) acc[k][l] = 0.f;
+  const int nvec = n / 8, nblk = nvec / 4;
+  for (int b = 0; b < nblk; ++b) {
+#pragma unroll
+    for (int t = 0; t < 32; ++t) acc[t / 8][t % 8] = __fadd_rn(acc[t / 8][t % 8], x[(int64_t)(b * 32 + t) * stride]);
+  }
+  for (int v = nblk * 4; v < nvec; ++v) {
+#pragma unroll
+    for (int l = 0; l < 8; ++l) acc[0][l] = __fadd_rn(x[(int64_t)(v * 8 + l) * stride], acc[0][l]);
+  }
+#pragma unroll
+  for (int k = 1; k < 4; ++k)
+#pragma unroll
+    for (int l = 0; l < 8; ++l) acc[0][l] = __fadd_rn(acc[0][l], acc[k][l]);
+  float fin = 0.f;
+  for (int i = nvec * 8; i < n; ++i) fin = __fadd_rn(fin, x[(int64_t)i * stride]);
+#pragma unroll
+  for (int l = 0; l < 8; ++l) fin = __fadd_rn(fin, acc[0][l]);
+  return fin;
+}
+
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int64_t align_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
 

@@ -11,7 +11,7 @@
 #include <cub/cub.cuh>
 #include <math_constants.h>
 
-#include "field.cuh"
+#include "edit.cuh"
 
 namespace nmb {
 
@@ -119,51 +119,6 @@ __global__ void coarse_z_kernel(int64_t R, int S, const float* __restrict__ near
   const float t = linspace01(s, S);
   z[i] = __fadd_rn(__fmul_rn(near[r], __fsub_rn(1.0f, t)), __fmul_rn(far[r], t));
   if (origin) origin[i] = s;   // sample s of ray r was evaluated as entry s of the neighbour arrays
-}
-
-// torch.sum over a contiguous fp32 row of n elements as ATen's CPU kernel computes it (SumKernel.cpp, the path
-// `weights.sum(dim=-1)` of rend_util.py:281 takes; checked against torch 2.11 for every n <= 255, AVX2 and AVX512
-// builds alike): the row is read as 8-lane vectors; four vector accumulators take vectors 4i, 4i+1, 4i+2, 4i+3, leftover
-// vectors go to accumulator 0, the accumulators are folded 0 += 1, 2, 3; then a scalar starts from 0, adds the tail
-// elements (n % 8) in order and finally the 8 lanes in order.  Rows shorter than 8 use four scalar accumulators in the
-// same pattern.  sample_pdf's u = 1 sample (searchsorted against a cdf that saturates at 1.0 or not) depends on these
-// bits, so the normalisation constant is reproduced exactly rather than summed sequentially.
-__device__ __forceinline__ float torch_row_sum(const float* __restrict__ x, int64_t stride, int n) {
-  if (n < 8) {
-    float a[4] = {0.f, 0.f, 0.f, 0.f};
-    const int q = n / 4;
-    if (q) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) a[k] = __fadd_rn(a[k], x[k * stride]);
-    }
-    for (int i = q * 4; i < n; ++i) a[0] = __fadd_rn(x[i * stride], a[0]);
-    a[0] = __fadd_rn(a[0], a[1]);
-    a[0] = __fadd_rn(a[0], a[2]);
-    return __fadd_rn(a[0], a[3]);
-  }
-  float acc[4][8];
-#pragma unroll
-  for (int k = 0; k < 4; ++k)
-#pragma unroll
-    for (int l = 0; l < 8; ++l) acc[k][l] = 0.f;
-  const int nvec = n / 8, nblk = nvec / 4;
-  for (int b = 0; b < nblk; ++b) {
-#pragma unroll
-    for (int t = 0; t < 32; ++t) acc[t / 8][t % 8] = __fadd_rn(acc[t / 8][t % 8], x[(int64_t)(b * 32 + t) * stride]);
-  }
-  for (int v = nblk * 4; v < nvec; ++v) {
-#pragma unroll
-    for (int l = 0; l < 8; ++l) acc[0][l] = __fadd_rn(x[(int64_t)(v * 8 + l) * stride], acc[0][l]);
-  }
-#pragma unroll
-  for (int k = 1; k < 4; ++k)
-#pragma unroll
-    for (int l = 0; l < 8; ++l) acc[0][l] = __fadd_rn(acc[0][l], acc[k][l]);
-  float fin = 0.f;
-  for (int i = nvec * 8; i < n; ++i) fin = __fadd_rn(fin, x[(int64_t)i * stride]);
-#pragma unroll
-  for (int l = 0; l < 8; ++l) fin = __fadd_rn(fin, acc[0][l]);
-  return fin;
 }
 
 // One up-sampling iteration for one ray (renderer.py:209-245 + rend_util.py:276-319 with det=True).
@@ -654,19 +609,32 @@ int64_t nmb_render_workspace_bytes(const nmb_render_cfg* cfg, int64_t rays_per_c
   return carve(nullptr, rays_per_chunk, P, n_new > 0 ? n_new : 1).total * (int64_t)sizeof(float) + 256;
 }
 
-int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_o, const float* rays_d, int64_t N,
-               int64_t rays_per_chunk, float* rgb, float* depth, float* acc, float* normals,
-               const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes, void* stream_) {
+int64_t nmb_render_edit_workspace_bytes(const nmb_render_cfg* cfg, const nmb_edit* edit, int64_t rays_per_chunk) {
+  const int64_t base = nmb_render_workspace_bytes(cfg, rays_per_chunk);
+  if (!edit || base == 0) return base;
+  // the edit pass runs over at most every mid-point of a chunk
+  const int64_t points = (int64_t)(cfg->N_samples + cfg->N_importance - 1) * rays_per_chunk;
+  return base + nmb::edit_carve(nullptr, points).total * (int64_t)sizeof(float);
+}
+
+}  // extern "C"
+
+static int render_impl(const nmb_field* f, const nmb_edit* edit, const nmb_render_cfg* cfg, const float* rays_o,
+                       const float* rays_d, int64_t N, int64_t rays_per_chunk, float* rgb, float* depth, float* acc,
+                       float* normals, const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes,
+                       void* stream_) {
   using namespace nmb;
   if (N <= 0) return 0;   // an empty shard: nothing to do (the output pointers of empty tensors are null)
   NMB_CHECK(f && cfg && rays_o && rays_d, "null argument");
+  NMB_CHECK(!edit || edit_grid(edit) == f->grid, "the edit was created for another main model's mesh grid");
+  NMB_CHECK(!edit || !cfg->sampling_only, "an edit changes colour only: sampling_only renders take nmb_render");
   NMB_CHECK(cfg->sampling_only ? (detail != nullptr) : (rgb && depth && acc), "null output");
   NMB_CHECK(rays_per_chunk > 0, "rays_per_chunk must be positive");
   NMB_CHECK(cfg->N_samples >= 2, "N_samples must be >= 2");
   NMB_CHECK(cfg->N_upsample_iters >= 0 && (cfg->N_upsample_iters == 0 || cfg->N_importance % cfg->N_upsample_iters == 0),
             "N_importance must be a multiple of N_upsample_iters");
   NMB_CHECK(!cfg->calc_normal || normals || cfg->sampling_only, "calc_normal needs a normals output");
-  NMB_CHECK(workspace_bytes >= nmb_render_workspace_bytes(cfg, rays_per_chunk), "workspace too small");
+  NMB_CHECK(workspace_bytes >= nmb_render_edit_workspace_bytes(cfg, edit, rays_per_chunk), "workspace too small");
   NMB_CHECK(N < (int64_t(1) << 31), "at most 2^31 - 1 rays per call (32-bit ray permutation)");
   NMB_CHECK(rays_per_chunk * (int64_t)(cfg->N_samples + cfg->N_importance) < (int64_t(1) << 31),
             "rays_per_chunk x samples per ray must stay below 2^31 (32-bit live-sample offsets)");
@@ -702,6 +670,8 @@ int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_
   for (int64_t c0 = 0; c0 < N; c0 += rays_per_chunk) {
     const int64_t R = (N - c0 < rays_per_chunk) ? (N - c0) : rays_per_chunk;
     Workspace w = carve(ws_aligned, R, P, n_new > 0 ? n_new : 1);
+    const EditScratch es = edit ? edit_carve(static_cast<float*>(ws_aligned) + w.total, (int64_t)(P - 1) * R)
+                                : EditScratch{};
     const int32_t* perm = perm_all + c0;   // chunk-local ray r  <->  caller's ray perm[r]
     const float* ro = w.orig;
     const unsigned rb = (unsigned)ceil_div(R, RT);
@@ -765,6 +735,7 @@ int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_
         in.R = R;
         rc = launch_color(f, in, Pn, w.rgb, stream);
         if (rc) return rc;
+        if (edit && (rc = apply_edit(edit, in, Pn, w.rgb, es, stream))) return rc;
       }
       return 0;
     };
@@ -815,7 +786,8 @@ int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_
     }
     midpoints_kernel<<<(unsigned)ceil_div(R * (P - 1), 256), 256, 0, stream>>>(R, P, w.z, w.zmid);
     NMB_LAUNCH_OK();
-    const bool need_mid_nabla = f->lay.use_nabla != 0;
+    // the colour MLPs of the main model or of an edit's reference models may take the mid-point nabla as an input
+    const bool need_mid_nabla = f->lay.use_nabla != 0 || (edit && edit_needs_nabla(edit));
     if (live_path) {
       // weights first, then only the samples that can contribute
       weights_kernel<<<rb, RT, 0, stream>>>(R, P, f->s, w.sdf, w.wbuf, w.nlive);
@@ -872,6 +844,7 @@ int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_
             in.dirs = w.live_dir;
             rc2 = launch_color(f, in, M, w.rgb, stream);
             if (rc2) return rc2;
+            if (edit && (rc2 = apply_edit(edit, in, M, w.rgb, es, stream))) return rc2;
           }
           return 0;
         };
@@ -909,6 +882,24 @@ int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_
     }
   }
   return 0;
+}
+
+extern "C" {
+
+int nmb_render(const nmb_field* f, const nmb_render_cfg* cfg, const float* rays_o, const float* rays_d, int64_t N,
+               int64_t rays_per_chunk, float* rgb, float* depth, float* acc, float* normals,
+               const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes, void* stream) {
+  return render_impl(f, nullptr, cfg, rays_o, rays_d, N, rays_per_chunk, rgb, depth, acc, normals, detail, workspace,
+                     workspace_bytes, stream);
+}
+
+int nmb_render_edit(const nmb_field* f, const nmb_edit* edit, const nmb_render_cfg* cfg, const float* rays_o,
+                    const float* rays_d, int64_t N, int64_t rays_per_chunk, float* rgb, float* depth, float* acc,
+                    float* normals, const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes,
+                    void* stream) {
+  NMB_CHECK(edit != nullptr, "null edit (plain renders take nmb_render)");
+  return render_impl(f, edit, cfg, rays_o, rays_d, N, rays_per_chunk, rgb, depth, acc, normals, detail, workspace,
+                     workspace_bytes, stream);
 }
 
 int nmb_upsample_step(const float* z, const float* sdf, int64_t N, int32_t n, int32_t n_new, float inv_s, float* z_new,

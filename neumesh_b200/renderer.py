@@ -2,7 +2,8 @@
 
 ``volume_render(rays_o, rays_d, model, **kwargs) -> (rgb, depth, extras)`` keeps the reference's keyword set
 (``renderer.py:105-135``; unknown kwargs are ignored as there).  A ``neumesh_b200.NeuMesh`` on CUDA with grad mode off
-is rendered by ``nmb_render`` (``csrc/render.cu``); every other case - arbitrary models such as the NeuS teacher,
+is rendered by ``nmb_render`` (``csrc/render.cu``), a texture-edit model (``TextureEditableNeuMesh`` or any object with
+its attributes) over such models by ``nmb_render_edit``; every other case - arbitrary models such as the NeuS teacher,
 grad-enabled training steps, ``perturb=True``, batched inputs with B > 1 - runs the generic torch-op path below, which
 follows the same algorithm through the model's public protocol.
 """
@@ -18,6 +19,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from .neumesh import NeuMesh
+from .texture_neumesh import edit_fused_supported, is_edit_model, packed_edit
 
 _WORKSPACES: "dict[tuple, torch.Tensor]" = {}
 DEFAULT_FUSED_CHUNK = 1 << 20  # rays per kernel chunk on the fused path (scratch ~19 KB / ray: 12 GB for an 800x800 frame)
@@ -47,9 +49,12 @@ def release_workspace(device: Optional[torch.device] = None) -> None:
 
 def fused_eligible(model, rays_o, *, batched, perturb, random_color_direction, use_view_dirs, N_samples, N_importance,
                    N_upsample_iters, samples_output) -> bool:
-    if not isinstance(model, NeuMesh) or torch.is_grad_enabled() or not rays_o.is_cuda:
+    if torch.is_grad_enabled() or not rays_o.is_cuda:
         return False
-    if not model.fused_supported() or not model.geometry_features.is_cuda:
+    if isinstance(model, NeuMesh):
+        if not model.fused_supported() or not model.geometry_features.is_cuda:
+            return False
+    elif not (is_edit_model(model) and getattr(model, "fused_render", True) and edit_fused_supported(model)):
         return False
     if random_color_direction or not use_view_dirs:
         return False
@@ -60,7 +65,7 @@ def fused_eligible(model, rays_o, *, batched, perturb, random_color_direction, u
     return True
 
 
-def render_fused(rays_o, rays_d, model: NeuMesh, *, obj_bounding_radius=1.0, calc_normal=False, white_bkgd=False,
+def render_fused(rays_o, rays_d, model, *, obj_bounding_radius=1.0, calc_normal=False, white_bkgd=False,
                  near_bypass=None, far_bypass=None, N_samples=64, N_importance=64, N_upsample_iters=4,
                  bounded_near_far=True, detailed_output=False, samples_output=False, chunk=None,
                  normalize_dirs=True, skip_dead_samples=True, min_chunk=None, perturb=False, perturb_u=None,
@@ -69,7 +74,10 @@ def render_fused(rays_o, rays_d, model: NeuMesh, *, obj_bounding_radius=1.0, cal
 
     ``perturb=True`` draws the up-sampling uniforms with ``torch.rand`` (``rend_util.py:292-295``); ``perturb_u``
     [N_upsample_iters, N, N_importance / N_upsample_iters] injects them instead (parity runs).  ``sampling_only=True``
-    runs the no-grad sampling cascade only and returns ``{"d_all", "implicit_surface", "near_far"}``."""
+    runs the no-grad sampling cascade only and returns ``{"d_all", "implicit_surface", "near_far"}``.
+
+    ``model`` is a ``NeuMesh`` or a texture-edit model (``texture_neumesh.packed_edit``): its main model drives the
+    cascade and ``nmb_render_edit`` blends the reference models' colours into every evaluated mid-point."""
     dev = rays_o.device
     o = rays_o.detach().reshape(-1, 3).float().contiguous()
     d = rays_d.detach().reshape(-1, 3).float().contiguous()
@@ -104,17 +112,25 @@ def render_fused(rays_o, rays_d, model: NeuMesh, *, obj_bounding_radius=1.0, cal
                          float(far_bypass or 0.0), int(bool(normalize_dirs)),
                          int(bool(skip_dead_samples) and not detailed_output), int(bool(sampling_only)),
                          u_dev.data_ptr() if u_dev is not None else None)
-    field = model.packed_field()
+    edit = None
+    if isinstance(model, NeuMesh):
+        geo = model
+    else:
+        if sampling_only:
+            raise ValueError("sampling_only renders the geometry only: pass the edit's main_model")
+        geo = model.main_model
+        edit = packed_edit(model)
+    field = geo.packed_field()
     L = _lib.lib()
     chunk = int(min(chunk or DEFAULT_FUSED_CHUNK, max(N, 1)))
     if min_chunk is not None:
         # the caller's ``rayschunk`` exists to bound memory (render.py passes 4096): never let the scratch of a chunk
         # take more than half of the device memory that is free right now, but never go below the caller's own chunk
-        per_ray = L.nmb_render_workspace_bytes(C.byref(cfg), 1 << 16) / float(1 << 16)
+        per_ray = L.nmb_render_edit_workspace_bytes(C.byref(cfg), edit, 1 << 16) / float(1 << 16)
         cached = _WORKSPACES.get((dev.type, dev.index, torch.cuda.current_stream(dev).cuda_stream))
         free = torch.cuda.mem_get_info(dev)[0] + (cached.numel() if cached is not None else 0)
         chunk = int(min(chunk, max(int(min_chunk), int(0.5 * free / per_ray))))
-    nbytes = L.nmb_render_workspace_bytes(C.byref(cfg), chunk)
+    nbytes = L.nmb_render_edit_workspace_bytes(C.byref(cfg), edit, chunk)
     ws = _workspace(dev, nbytes)
     P = N_samples + (N_importance if N_upsample_iters > 0 else 0)
     if sampling_only:
@@ -139,18 +155,17 @@ def render_fused(rays_o, rays_d, model: NeuMesh, *, obj_bounding_radius=1.0, cal
             det_t["implicit_nablas"] = torch.empty(N, P, 3, device=dev)
         det = _lib.RenderDetail(*[det_t[k].data_ptr() if k in det_t else None for k in
                                   ("d_all", "implicit_surface", "implicit_nablas", "radiance", "sdf_mid", "near_far")])
+    args = (C.byref(cfg), _lib.ptr(o), _lib.ptr(d), N, chunk, _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(acc),
+            _lib.ptr(normals), C.byref(det) if det is not None else None, _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
     with torch.cuda.device(dev):
-        _lib.check(L.nmb_render(field, C.byref(cfg), _lib.ptr(o), _lib.ptr(d), N, chunk, _lib.ptr(rgb),
-                                _lib.ptr(depth), _lib.ptr(acc), _lib.ptr(normals),
-                                C.byref(det) if det is not None else None, _lib.ptr(ws), ws.numel(),
-                                _lib.stream_ptr(dev)))
+        _lib.check(L.nmb_render(field, *args) if edit is None else L.nmb_render_edit(field, edit, *args))
     out = OrderedDict([("rgb", rgb), ("depth_volume", depth), ("mask_volume", acc)])
     if calc_normal:
         out["normals_volume"] = normals
     if detailed_output:
         # same quantities the reference returns (renderer.py:335-348), recomputed from the exported samples
         sdf, z = det_t["implicit_surface"], det_t["d_all"]
-        cdf = torch.sigmoid(sdf * model.forward_s().detach())
+        cdf = torch.sigmoid(sdf * geo.forward_s().detach())
         alpha = ((cdf[..., :-1] - cdf[..., 1:]) / (cdf[..., :-1] + 1e-10)).clamp_min(0)
         if calc_normal:
             out["implicit_nablas"] = det_t["implicit_nablas"]
