@@ -111,6 +111,130 @@ def icosphere_mesh(level: int = 5, radius: float = 0.5, bump: float = 0.05, seed
     return mesh.compute_vertex_normals()
 
 
+# Meshes unlike the icosphere, for the tests of everything whose correctness depends on the mesh's shape (the exact
+# octree walks, the shell certificate, the bounded near / far scan).  Scans and edited meshes are open, non-convex,
+# unevenly dense, and may carry duplicate or exactly coplanar vertices; each generator below stresses one of these.
+def _finish(p: np.ndarray, f: np.ndarray) -> SynthMesh:
+    p = np.ascontiguousarray(p).astype(np.float32).astype(np.float64)
+    mesh = SynthMesh(vertices=p, triangles=np.ascontiguousarray(f).astype(np.int32), vertex_normals=np.zeros_like(p))
+    return mesh.compute_vertex_normals()
+
+
+def _rotation(rng) -> np.ndarray:
+    q, r = np.linalg.qr(rng.normal(size=(3, 3)))
+    q = q * np.sign(np.diag(r))[None, :]
+    if np.linalg.det(q) < 0:
+        q[:, 0] = -q[:, 0]
+    return q
+
+
+def _drop_vertices(v: np.ndarray, f: np.ndarray, keep: np.ndarray):
+    """Keep the faces whose three vertices are kept, then drop the vertices no face references."""
+    f = f[keep[f].all(axis=1)]
+    used = np.zeros(v.shape[0], dtype=bool)
+    used[f.reshape(-1)] = True
+    new_id = np.cumsum(used) - 1
+    return v[used], new_id[f]
+
+
+def _grid_faces(nu: int, nv: int, wrap_u: bool, wrap_v: bool) -> np.ndarray:
+    """Two triangles per quad of an nu x nv vertex grid (vertex (i, j) at i * nv + j)."""
+    iu = np.arange(nu if wrap_u else nu - 1)
+    jv = np.arange(nv if wrap_v else nv - 1)
+    i, j = np.meshgrid(iu, jv, indexing="ij")
+    i, j = i.reshape(-1), j.reshape(-1)
+    i1, j1 = (i + 1) % nu, (j + 1) % nv
+    a, b, c, d = i * nv + j, i1 * nv + j, i1 * nv + j1, i * nv + j1
+    return np.concatenate([np.stack([a, b, c], 1), np.stack([a, c, d], 1)], axis=0)
+
+
+def open_bowl(level: int = 6, radius: float = 0.45, seed: int = 0, cap: float = 0.55,
+              centre=(0.12, -0.08, 0.05)) -> SynthMesh:
+    """A jittered icosphere with the cap dir_z < -cap cut off: an open boundary, off-centre, with its concave inside
+    facing the spiral track's centre camera (which looks down +z from z = -2.5)."""
+    m = icosphere_mesh(level, radius=1.0, bump=0.0, seed=seed)
+    v = m.vertices / np.linalg.norm(m.vertices, axis=1, keepdims=True)
+    v, f = _drop_vertices(v, m.triangles.astype(np.int64), v[:, 2] >= -cap)
+    return _finish(v * radius + np.asarray(centre, dtype=np.float64), f)
+
+
+def torus(R: float = 0.55, r: float = 0.15, nu: int = 256, nv: int = 64, seed: int = 0) -> SynthMesh:
+    """A tilted, jittered torus: not star-shaped, rays pass through the hole, some rays cross it twice."""
+    rng = np.random.default_rng(seed)
+    u = (np.arange(nu)[:, None] + 0.3 * rng.uniform(-1, 1, size=(nu, nv))) * (2 * np.pi / nu)
+    w = (np.arange(nv)[None, :] + 0.3 * rng.uniform(-1, 1, size=(nu, nv))) * (2 * np.pi / nv)
+    p = np.stack([(R + r * np.cos(w)) * np.cos(u), (R + r * np.cos(w)) * np.sin(u), r * np.sin(w)], -1).reshape(-1, 3)
+    return _finish(p @ _rotation(rng).T, _grid_faces(nu, nv, True, True))
+
+
+def double_sheet(radius: float = 0.6, spacing: float = 0.01, gap: float = 0.03, seed: int = 0) -> SynthMesh:
+    """Two jittered, tilted disks `gap` apart with opposite normals, each inside the other's 0.1 shell: a query between
+    them has neighbours on both sheets, whose indicator vectors point in opposite directions."""
+    rng = np.random.default_rng(seed)
+    n = int(round(2 * radius / spacing)) + 1
+    x = np.linspace(-radius, radius, n)
+    gx, gy = np.meshgrid(x, x, indexing="ij")
+    base = np.stack([gx.reshape(-1), gy.reshape(-1)], -1)
+    f0 = _grid_faces(n, n, False, False)
+    keep = (base ** 2).sum(1) <= radius * radius
+    vs, fs = [], []
+    for k, (z, flip) in enumerate(((0.5 * gap, False), (-0.5 * gap, True))):
+        xy = base + rng.uniform(-0.3, 0.3, size=base.shape) * spacing
+        p = np.concatenate([xy, np.full((xy.shape[0], 1), z)], 1)
+        p, f = _drop_vertices(p, f0, keep)
+        if flip:
+            f = f[:, ::-1]
+        fs.append(f + sum(q.shape[0] for q in vs))
+        vs.append(p)
+    return _finish(np.concatenate(vs) @ _rotation(rng).T, np.concatenate(fs))
+
+
+def lattice_plane(n: int = 257, spacing: float = 1.0 / 256) -> SynthMesh:
+    """An n x n grid at z = 0 with a power-of-two spacing: every coordinate is exact in fp32, so squared distances tie
+    exactly everywhere (2-, 4- and 8-way ties at cell centres and edge midpoints) and every node has a zero-thickness
+    disc."""
+    x = (np.arange(n) - (n - 1) // 2) * spacing
+    gx, gy = np.meshgrid(x, x, indexing="ij")
+    p = np.stack([gx.reshape(-1), gy.reshape(-1), np.zeros(n * n)], -1)
+    return _finish(p, _grid_faces(n, n, False, False))
+
+
+def clustered(seed: int = 0, n_dup: int = 200) -> SynthMesh:
+    """A coarse sphere (level 3, radius 0.5), a dense level-6 icosphere of radius 0.02 sitting on its surface, and
+    `n_dup` exact copies of one of the dense vertices (unreferenced by any face).  The cluster packs ~100 vertices into
+    each finest octree cell, so the deepest leaves hold far more than LEAF_MAX points."""
+    coarse = icosphere_mesh(3, radius=0.5, bump=0.02, seed=seed)
+    dense = icosphere_mesh(6, radius=0.02, bump=0.0, seed=seed + 1)
+    c = coarse.vertices[7]
+    v = np.concatenate([coarse.vertices, dense.vertices + c])
+    f = np.concatenate([coarse.triangles, dense.triangles + coarse.vertices.shape[0]])
+    dup = np.repeat(v[coarse.vertices.shape[0] + 5][None], n_dup, axis=0)
+    return _finish(np.concatenate([v, dup]), f)
+
+
+def fan_mesh(V: int, seed: int = 0) -> SynthMesh:
+    """A tiny triangle fan: one apex and V - 1 rim vertices at seeded radii and heights."""
+    rng = np.random.default_rng(seed)
+    a = np.sort(rng.uniform(0, 2 * np.pi, size=V - 1))
+    rr = rng.uniform(0.3, 0.8, size=V - 1)
+    rim = np.stack([rr * np.cos(a), rr * np.sin(a), rng.uniform(-0.3, 0.3, size=V - 1)], -1)
+    p = np.concatenate([np.array([[0.0, 0.0, 0.2]]), rim])
+    i = np.arange(1, V)
+    f = np.stack([np.zeros(V - 1, dtype=np.int64), i, np.where(i + 1 < V, i + 1, 1)], 1)
+    return _finish(p, f)
+
+
+FAR_BOWL_OFFSET = (100.0, -37.5, 12.25)
+FAR_BOWL_SCALE = 1.0 / 64
+
+
+def far_bowl(seed: int = 0) -> SynthMesh:
+    """``open_bowl`` scaled by 1/64 and moved to about (100, -37.5, 12.25): the fp32 margins of the walk's bounds at
+    coordinates whose ulp is ~1000 times coarser than at the unit scale, relative to the mesh."""
+    m = open_bowl(seed=seed)
+    return _finish(m.vertices * FAR_BOWL_SCALE + np.asarray(FAR_BOWL_OFFSET), m.triangles)
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # model parameters
 # ----------------------------------------------------------------------------------------------------------------

@@ -48,7 +48,7 @@ def inverse_cdf_samples(bins, weights, n, u=None):
 
 def mesh_bounded_near_far(field, o, d, near, far, n_grid=256, thresh=0.1):
     """renderer.py:66-102."""
-    t = torch.linspace(0, 1, n_grid)
+    t = torch.linspace(0, 1, n_grid).to(near.device)   # the CPU values, also for tensors on a GPU
     depth = (near * (1 - t) + far * t)[..., None]  # [N, G, 1]
     pts = o[:, None, :] + depth * d[:, None, :]
     ds, _, _ = field.compute_distance(pts)

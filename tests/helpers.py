@@ -54,6 +54,145 @@ def sample_points(n, seed=0):
     return dirs * radii[:, None], view
 
 
+RGB_TOL, DEPTH_TOL = 1e-4, 1e-5
+
+
+def kernel_normalize(d):
+    """The fused renderer's ray direction (``ray_setup_kernel``): d / max(sqrt((x*x + y*y) + z*z), 1e-12), every operation
+    rounded separately.  ``F.normalize`` reduces the norm in another order and differs in the last bit for ~9 % of the
+    directions of a spiral frame, which moves a sample point by an ulp - enough to switch a near-tied neighbour."""
+    n = ((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]).sqrt().clamp_min(1e-12)
+    return d / n[..., None]
+
+
+def teacher_forced(f, o, d, z_all, calc_normal, white_bkgd):
+    """Oracle field + oracle compositing at given sample depths (renderer.py:264-333), at the sample points of the fused
+    renderer (its direction formula, ``kernel_normalize``)."""
+    from oracle import render as orender
+    dn = kernel_normalize(d)
+    pts = o[:, None, :] + z_all[..., None] * dn[:, None, :]
+    z_mid = 0.5 * (z_all[..., 1:] + z_all[..., :-1])
+    pm = o[:, None, :] + z_mid[..., None] * dn[:, None, :]
+    if calc_normal:
+        sdf, nab = f.forward_with_nablas(pts)
+    else:
+        sdf, nab = f.forward_density_only(pts), None
+    sdf = sdf.squeeze(-1)
+    cdf = torch.sigmoid(sdf * f.forward_s())
+    alpha = ((cdf[..., :-1] - cdf[..., 1:]) / (cdf[..., :-1] + 1e-10)).clamp_min(0)
+    _, rad = f.forward(pm, dn[:, None, :].expand_as(pm))
+    w = orender.transmittance_weights(alpha)
+    rgb = (w[..., None] * rad).sum(-2)
+    acc = w.sum(-1)
+    depth = (w / (acc[..., None] + 1e-10) * z_mid).sum(-1)
+    if white_bkgd:
+        rgb = rgb + (1 - acc[..., None])
+    normals = None
+    if calc_normal:
+        nn_ = torch.nn.functional.normalize(nab, dim=-1)
+        normals = (nn_[..., :-1, :] * w[..., None]).sum(-2)
+    return rgb, depth, acc, normals
+
+
+def check_render_teacher_forced(model, mesh, cfg, sd, f, o, d, tag, ties_by_neighbours=False,
+                                depth_acc_tol=DEPTH_TOL):
+    """Render o, d with the CUDA path, then hold its composited outputs to the fp32 oracle and to float64 evaluated at
+    the CUDA path's own sample depths, and its per-sample sdf / nabla to the oracle field at those depths.
+
+    ``depth_acc_tol`` is the bar on depth * acc against the fp32 oracle; the bar against float64 (CUDA depth error on
+    solid rays no worse than 5 x the oracle's own + 4e-6) always holds.
+
+    ``ties_by_neighbours``: instead of bounding the error of the few samples on an exact 8th / 9th distance tie, find
+    them (the oracle's and the CUDA path's neighbour lists differ while their squared distances are identical), require
+    every other sample within the per-sample bars, and leave the rays through a tie sample out of the composited bars.
+    On meshes whose neighbouring vertices carry very different indicator vectors (a flip between two facing sheets) a
+    tie decides the sdf by more than the icosphere's 2e-3."""
+    import neumesh_b200 as nb
+    dev = next(model.parameters()).device
+    N = o.shape[0]
+    kw = dict(calc_normal=True, white_bkgd=True, bounded_near_far=True)
+    with torch.no_grad():
+        rgb, depth, ex = nb.volume_render(o.to(dev), d.to(dev), model, detailed_output=True, **kw)
+    z_all = ex["d_all"].cpu()
+    assert z_all.shape == (N, 128) and (z_all[:, 1:] >= z_all[:, :-1]).all()
+    r_rgb, r_depth, r_acc, r_n = teacher_forced(f, o, d, z_all, True, True)
+    f64 = oracle_field(mesh, cfg, sd, torch.float64)
+    t_rgb, t_depth, t_acc, t_n = teacher_forced(f64, o.double(), d.double(), z_all.double(), True, True)
+    # per-sample outputs at the exported depths: every sample's sdf / nabla must be THE field at that depth - including
+    # the first sample of a ray that each deterministic up-sampling iteration draws again (u = 0) and the fused cascade
+    # copies instead of evaluating
+    dn_ = kernel_normalize(d)
+    pts_all = o[:, None, :] + z_all[..., None] * dn_[:, None, :]
+    o_sdf, o_nab = f.forward_with_nablas(pts_all)
+    err_s = (ex["implicit_surface"].cpu() - o_sdf.squeeze(-1)).abs()
+    err_n = (ex["implicit_nablas"].cpu() - o_nab).abs().amax(-1)
+    n_dup = int((z_all[:, 1:] == z_all[:, :-1]).sum())
+    bad = (err_s > 5e-6) | (err_n > 1.5e-4)
+    print(f"[{tag}] per-sample at d_all: sdf max {err_s.max():.3e} nabla max {err_n.max():.3e}, {int(bad.sum())} of "
+          f"{bad.numel()} samples outside (5e-6, 1.5e-4); {n_dup} duplicated depths")
+    assert n_dup >= 4 * N * 0.9, "deterministic up-sampling re-draws the first sample of every ray"
+    keep = torch.ones(N, dtype=torch.bool)
+    if ties_by_neighbours:
+        from oracle import knn as oknn
+        flat = pts_all.reshape(-1, 3)
+        _, idx_o, _ = f.compute_distance(flat)
+        with torch.no_grad():
+            _, idx_c, _ = model.compute_distance(flat.to(dev))
+        idx_c = idx_c.cpu()
+        tie = (idx_o != idx_c).any(-1)
+        pv = torch.from_numpy(mesh.vertices).float()
+        assert torch.equal(oknn._sq_dist_f32(flat[tie], pv, idx_o[tie]), oknn._sq_dist_f32(flat[tie], pv, idx_c[tie]))
+        tie = tie.reshape(N, -1)
+        other = bad & ~tie
+        print(f"[{tag}] {int(tie.sum())} samples on an exact 8th / 9th distance tie, {int(other.sum())} other samples "
+              f"outside the bars (sdf {err_s[other].tolist()}, nabla {err_n[other].tolist()}); "
+              f"{int(tie.any(1).sum())} rays through a tie left out of the composited bars")
+        # a tie sample is copied into up to 5 sample slots (the re-drawn first sample): measured 33 / 93 / 98 tie samples
+        # of 204 800 on the torus / bowl / double sheet, so at most 1 in 1 000 samples
+        assert int(tie.sum()) <= bad.numel() // 1000 and int(other.sum()) == 0
+        keep = ~tie.any(1)
+    else:
+        # a handful of samples sit on an exact fp32 distance tie between the 8th and 9th neighbour, where the chosen
+        # vertex is implementation-defined (measured: sdf 2.8e-4 on the same sample with every engine;
+        # __graft_entry__.smoke masks them by comparing neighbour lists).  A wrong copy would touch >= 1 sample per ray
+        # and iteration (4 per ray).
+        assert int(bad.sum()) <= 64 and err_s.max().item() <= 2e-3
+    rgb, depth, r_rgb, r_depth, t_rgb, t_depth = (t[keep] for t in (rgb.cpu(), depth.cpu(), r_rgb, r_depth, t_rgb, t_depth))
+    r_acc, r_n = r_acc[keep], r_n[keep]
+    ex = {k: ex[k].cpu()[keep] for k in ("mask_volume", "normals_volume")}
+    acc = ex["mask_volume"].cpu()
+    solid = acc >= 0.5
+    e_rgb = (rgb.cpu() - r_rgb).abs().max().item()
+    dd = (depth.cpu() - r_depth).abs()
+    e_acc = (acc - r_acc).abs().max().item()
+    e_nrm = (ex["normals_volume"].cpu() - r_n).abs().max().item()
+    # accuracy against float64 "truth" at the same samples: CUDA path vs the fp32 oracle (= the reference's arithmetic)
+    c_rgb = (rgb.cpu().double() - t_rgb).abs().max().item()
+    o_rgb = (r_rgb.double() - t_rgb).abs().max().item()
+    c_dep = (depth.cpu().double() - t_depth).abs()[solid].max().item()
+    o_dep = (r_depth.double() - t_depth).abs()[solid].max().item()
+    print(f"[{tag}] teacher-forced vs oracle(fp32): rgb {e_rgb:.3e}  depth on solid rays (acc>=0.5, "
+          f"{int(solid.sum())} rays): max {dd[solid].max():.3e} p99 {dd[solid].quantile(0.99):.3e} "
+          f"median {dd[solid].median():.3e};  depth*acc all rays {(dd * acc.clamp_min(1e-6)).max():.3e};  "
+          f"depth all rays {dd.max():.3e};  acc {e_acc:.3e};  normals {e_nrm:.3e}")
+    print(f"[{tag}] teacher-forced vs float64 truth: rgb CUDA {c_rgb:.3e} / oracle(fp32) {o_rgb:.3e};  "
+          f"depth(solid) CUDA {c_dep:.3e} / oracle(fp32) {o_dep:.3e}")
+    # RGB: the north-star bar, every ray.
+    assert e_rgb <= RGB_TOL
+    # Depth: the reference's depth = sum(w / (sum(w) + 1e-10) * z) divides by the accumulated opacity, so it is
+    # ill-conditioned as acc -> 0 (grazing rays).  Two fp32 evaluations of the SAME sdf network (MKL sgemm vs these
+    # kernels) differ by ~1e-6 in sdf, which the sharpness s ~ 245 amplifies.  Also asserted: the CUDA path's distance to
+    # the float64 truth is of the same order as that of the reference's own fp32 arithmetic.
+    # the depth bar holds at p99 of the rays with acc >= 0.5 and within 2x on the worst of them, and on the low-opacity
+    # rays (where depth = sum(w z) / sum(w) is ill-conditioned as sum(w) -> 0) for depth * acc, the quantity that is
+    # composited into an image
+    assert dd[solid].quantile(0.99).item() <= DEPTH_TOL
+    assert dd[solid].max().item() <= 2 * DEPTH_TOL
+    assert (dd * acc.clamp_min(1e-6)).max().item() <= depth_acc_tol
+    assert c_dep <= 5 * o_dep + 4e-6 and c_rgb <= 2 * o_rgb + 2e-5
+    assert e_acc <= 2.7e-4 and e_nrm <= 2.5e-4
+
+
 from oracle.mesh_grid import OracleMeshGrid  # noqa: E402,F401  (CPU stand-in for MeshGrid; test infrastructure)
 
 
