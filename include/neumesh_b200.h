@@ -98,6 +98,10 @@ int nmb_field_create(const nmb_grid* g, const nmb_field_desc* desc, int mlp_engi
 void nmb_field_destroy(nmb_field* f);
 /* re-pack after the caller changed parameter values in place (same shapes) */
 int nmb_field_update(nmb_field* f, const nmb_field_desc* desc, void* stream);
+/* Whether the fused kernels take this configuration on this engine: 0, or 2 with the reason in nmb_last_error().
+ * Reads only the integer fields of desc (no pointer is dereferenced) and makes no CUDA call, so it also answers on a host
+ * without a GPU.  nmb_field_create and nmb_field_update refuse exactly what it refuses. */
+int nmb_field_check(const nmb_field_desc* desc, int mlp_engine);
 
 /* NeuMesh.forward_density_only / forward_with_nablas (neumesh.py:140-154): sdf [M]; nabla [M,3] nullable. */
 int nmb_field_sdf(const nmb_field* f, const float* xyz /*[M,3]*/, int64_t M, float* sdf, float* nabla, void* stream);

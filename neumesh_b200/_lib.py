@@ -58,6 +58,7 @@ SIGNATURES = {
     "nmb_grid_order": (_P, [_P]),
     "nmb_knn": (C.c_int, [_P, _P, _I64, C.c_int, _F, _P, _P, _P]),
     "nmb_mesh_distance": (C.c_int, [_P, _P, _F, _P, _I64, _P, _P, _P, _P, _P]),
+    "nmb_field_check": (C.c_int, [C.POINTER(FieldDesc), C.c_int]),
     "nmb_field_create": (C.c_int, [_P, C.POINTER(FieldDesc), C.c_int, _P, C.POINTER(_P)]),
     "nmb_field_destroy": (None, [_P]),
     "nmb_field_update": (C.c_int, [_P, C.POINTER(FieldDesc), _P]),

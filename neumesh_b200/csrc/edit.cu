@@ -251,7 +251,6 @@ static int edit_check(const nmb_field* main_field, int32_t n_ref, const nmb_fiel
     const nmb_field* r = ref_fields[i];
     NMB_CHECK(r != nullptr, "null reference field");
     NMB_CHECK(r->lay.Fc == color_dim, "every reference field's color_dim must equal the code table width");
-    NMB_CHECK(r->lay.off_ft <= 64 || r->engine == 1, "reference field's colour head block is wider than 64 columns");
   }
   return 0;
 }

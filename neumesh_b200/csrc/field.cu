@@ -69,6 +69,28 @@ static FieldLayout make_layout(const nmb_field_desc* d) {
   return L;
 }
 
+// Every configuration limit of the fused kernels, from the descriptor's integer fields and the engine only (no CUDA
+// call).  A packed field has passed it, so the launchers do not check again.
+static int check_field(const nmb_field_desc* d, int engine) {
+  NMB_CHECK(engine >= 0 && engine <= 2, "mlp_engine must be 0 (tensor-core 3xTF32), 1 (fp32) or 2 (tensor-core fp16x3)");
+  NMB_CHECK(d->W == MLP_W, "fused kernels are specialised for W = 256");
+  NMB_CHECK(d->geometry_dim >= FEAT && d->geometry_dim % FEAT == 0 && d->color_dim >= FEAT && d->color_dim % FEAT == 0,
+            "fused kernels need vertex code widths that are multiples of 32");
+  NMB_CHECK(engine != 1 || (d->geometry_dim == FEAT && d->color_dim == FEAT),
+            "the fp32 engine is specialised for 32-d vertex codes (use a tensor-core engine)");
+  NMB_CHECK(d->D_density >= 1 && d->D_density < MAX_LAYERS && d->D_color >= 1 && d->D_color < MAX_LAYERS,
+            "unsupported MLP depth");
+  NMB_CHECK(d->multires_d >= 0 && d->multires_fg >= 0 && d->multires_ft >= 0 && d->multires_view >= 0,
+            "identity embedders (multires < 0) are not supported by the fused kernels");
+  NMB_CHECK(engine != 2 || d->multires_d <= F16_MAX_MULTIRES_D,
+            "multires_d > 16 overflows the fp16 engine's tangent operands (use the 3xTF32 engine)");
+  const FieldLayout L = make_layout(d);
+  NMB_CHECK(engine != 1 || (L.K0g <= 256 && L.K0c <= 256), "first-layer width exceeds the fp32 engine's 256-column tile");
+  NMB_CHECK(engine == 1 || (L.off_fg <= 64 && L.off_ft <= 64),
+            "head block wider than 64 columns (the tensor-core engines' limit)");
+  return 0;
+}
+
 // reference column of each of our first-layer columns (-1 = padding)
 static std::vector<int32_t> geo_colmap(const FieldLayout& L) {
   std::vector<int32_t> m(L.K0g, -1);
@@ -130,28 +152,17 @@ static int pack_ffma(const float* const* v, const float* const* g, const float* 
 
 static int pack_field(const nmb_field_desc* d, nmb_field* f, cudaStream_t stream) {
   const nmb_grid* g = f->grid;
-  NMB_CHECK(d->W == MLP_W, "fused kernels are specialised for W = 256");
-  NMB_CHECK(d->geometry_dim >= FEAT && d->geometry_dim % FEAT == 0 && d->color_dim >= FEAT && d->color_dim % FEAT == 0,
-            "fused kernels need vertex code widths that are multiples of 32");
-  NMB_CHECK(f->engine != 1 || (d->geometry_dim == FEAT && d->color_dim == FEAT),
-            "the fp32 engine is specialised for 32-d vertex codes (use a tensor-core engine)");
-  NMB_CHECK(d->D_density >= 1 && d->D_density < MAX_LAYERS && d->D_color >= 1 && d->D_color < MAX_LAYERS,
-            "unsupported MLP depth");
-  NMB_CHECK(d->multires_d >= 0 && d->multires_fg >= 0 && d->multires_ft >= 0 && d->multires_view >= 0,
-            "identity embedders (multires < 0) are not supported by the fused kernels");
-  NMB_CHECK(f->engine != 2 || d->multires_d <= F16_MAX_MULTIRES_D,
-            "multires_d > 16 overflows the fp16 engine's tangent operands (use the 3xTF32 engine)");
+  int rc = check_field(d, f->engine);
+  if (rc) return rc;
   f->lay = make_layout(d);
   f->shell_valid = false;
   f->shell = ShellGrid{};
-  NMB_CHECK(f->engine != 1 || (f->lay.K0g <= 256 && f->lay.K0c <= 256),
-            "first-layer width exceeds the fp32 engine's 256-column tile");
   f->w1 = d->indicator_weight;
   f->s = d->s;
   NMB_CUDA_OK(f->indicator.alloc(g->V));
   NMB_CUDA_OK(f->fg.alloc(g->V * f->lay.Fg));
   NMB_CUDA_OK(f->fc.alloc(g->V * f->lay.Fc));
-  int rc = permute_indicator(g, d->indicator_vector, f->indicator.p, stream);
+  rc = permute_indicator(g, d->indicator_vector, f->indicator.p, stream);
   if (rc) return rc;
   const unsigned blocks = (unsigned)ceil_div(g->V * 32, 256);
   permute_table_kernel<<<blocks, 256, 0, stream>>>(d->geometry_features, g->order.p, g->V, f->lay.Fg, f->fg.p);
@@ -203,10 +214,9 @@ int nmb_field_create(const nmb_grid* g, const nmb_field_desc* desc, int mlp_engi
   if (!out) return 2;
   *out = nullptr;
   NMB_CHECK(g != nullptr && desc != nullptr, "null grid / descriptor");
-  NMB_CHECK(mlp_engine >= 0 && mlp_engine <= 2, "mlp_engine must be 0 (tensor-core 3xTF32), 1 (fp32) or 2 (tensor-core fp16x3)");
   nmb_field* f = new nmb_field();
   f->grid = g;
-  f->engine = mlp_engine;
+  f->engine = mlp_engine;   // pack_field validates it with the descriptor
   int rc = nmb::pack_field(desc, f, static_cast<cudaStream_t>(stream));
   if (rc) {
     delete f;
@@ -214,6 +224,11 @@ int nmb_field_create(const nmb_grid* g, const nmb_field_desc* desc, int mlp_engi
   }
   *out = f;
   return 0;
+}
+
+int nmb_field_check(const nmb_field_desc* desc, int mlp_engine) {
+  NMB_CHECK(desc != nullptr, "null descriptor");
+  return nmb::check_field(desc, mlp_engine);
 }
 
 void nmb_field_destroy(nmb_field* f) { delete f; }

@@ -241,13 +241,11 @@ static int launch_ffma(const nmb_field* f, const MlpFfma& mlp, const FieldIn& in
 }
 
 int launch_geo_ffma(const nmb_field* f, const FieldIn& in, int64_t P, float* sdf, float* nabla, cudaStream_t stream) {
-  NMB_CHECK(f->lay.Fg == FEAT && f->lay.K0g <= 256, "the fp32 engine is specialised for 32-d vertex codes");
   if (nabla) return launch_ffma<1>(f, f->geo_f, in, P, sdf, nabla, stream);
   return launch_ffma<0>(f, f->geo_f, in, P, sdf, nullptr, stream);
 }
 
 int launch_color_ffma(const nmb_field* f, const FieldIn& in, int64_t P, float* rgb, cudaStream_t stream) {
-  NMB_CHECK(f->lay.Fc == FEAT && f->lay.K0c <= 256, "the fp32 engine is specialised for 32-d vertex codes");
   return launch_ffma<2>(f, f->col_f, in, P, rgb, nullptr, stream);
 }
 

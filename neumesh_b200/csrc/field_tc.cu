@@ -845,7 +845,6 @@ template <int MODE, bool F16>
 static int launch_tc(const nmb_field* f, const MlpFfma& fm, const MlpTc& tm, const FieldIn& in, int64_t P, float* out0,
                      float* out1, cudaStream_t stream) {
   if (P <= 0) return 0;
-  NMB_CHECK(f->lay.off_fg <= 64 && f->lay.off_ft <= 64, "head block wider than 64 columns");
   tc::Params prm;
   prm.lay = f->lay;
   prm.in = in;

@@ -62,27 +62,6 @@ def _mlp_stack(make_linear, act, in_dim, width, depth):
 MLP_ENGINES = {"tcgen05": 0, "fp32": 1, "tcgen05_f16": 2}
 DEFAULT_MLP_ENGINE = "tcgen05_f16"
 
-# Limits of the fused kernels, mirrored from the library so that unsupported configurations take the torch-op path
-# instead of failing at pack or launch time.
-MAX_LAYERS = 8            # csrc/field.cuh MAX_LAYERS: D_density and D_color are at most MAX_LAYERS - 1
-TC_MAX_HEAD = 64          # csrc/field_tc.cu launch_tc: the head block (columns before the vertex codes) is <= 64 wide
-FFMA_MAX_K0 = 256         # csrc/field.cu pack_field: the fp32 engine's first layer fits one 256-column tile
-F16_MAX_MULTIRES_D = 16   # csrc/field.cuh F16_MAX_MULTIRES_D: fp16 operands hold the tangent seed 2^(L-1) (<= 65504)
-
-
-def _align16(n: int) -> int:
-    return (n + 15) // 16 * 16
-
-
-def _first_layer_widths(cfg: dict, enable_nablas_input: bool):
-    """(head_g, K0g, head_c, K0c): widths of the geometry / colour head blocks and first layers as the library packs
-    them (csrc/field.cu make_layout)."""
-    ch_d = 1 + 2 * cfg["multires_d"]
-    head_g = _align16(ch_d)
-    head_c = _align16(ch_d + (3 if enable_nablas_input else 0) + 3 * (1 + 2 * cfg["multires_view"]))
-    return (head_g, _align16(head_g + cfg["geometry_dim"] * (1 + 2 * cfg["multires_fg"])),
-            head_c, _align16(head_c + cfg["color_dim"] * (1 + 2 * cfg["multires_ft"])))
-
 
 class NeuMesh(nn.Module):
     def __init__(self, mesh_grid, D_density: int, D_color: int, W: int, geometry_dim: int, color_dim: int,
@@ -123,6 +102,7 @@ class NeuMesh(nn.Module):
         self.mlp_engine = mlp_engine
         self._field = None
         self._field_key = None
+        self._field_check = {}        # mlp_engine -> None or the library's reason for refusing _cfg on that engine
         # grad-enabled queries on CUDA run the fused training op (train_ops.FusedFieldFn); False = torch-op path
         self.fused_train = True
         self._train_prims = None      # tests inject a torch implementation of the kernel interface here (CPU)
@@ -138,21 +118,34 @@ class NeuMesh(nn.Module):
         return [self.views_linears[0]] + [self.views_linears[i][0] for i in range(2, len(self.views_linears))] + \
             [self.color_linear[0]]
 
-    def fused_supported(self) -> bool:
+    def _field_desc(self):
+        """``nmb_field_desc`` with the configuration's integer fields set: all ``nmb_field_check`` reads."""
         c = self._cfg
-        wide = self.mlp_engine != "fp32"         # the fp32 engine is specialised for 32-d codes
-        dims_ok = all(d >= 32 and d % 32 == 0 and (wide or d == 32) for d in (c["geometry_dim"], c["color_dim"]))
-        if not (c["W"] == 256 and dims_ok and c["input_view_dim"] == 3
-                and c["input_d_dim"] == 1 and min(c["multires_d"], c["multires_fg"], c["multires_ft"],
-                                                  c["multires_view"]) >= 0
-                and all(1 <= c[k] < MAX_LAYERS for k in ("D_density", "D_color"))
-                and hasattr(self.mesh_grid, "grid") and hasattr(self.mesh_grid.grid, "handle")):
-            return False
-        head_g, k0g, head_c, k0c = _first_layer_widths(c, self.enable_nablas_input)
-        if not wide:
-            return k0g <= FFMA_MAX_K0 and k0c <= FFMA_MAX_K0
-        return (head_g <= TC_MAX_HEAD and head_c <= TC_MAX_HEAD
-                and (self.mlp_engine != "tcgen05_f16" or c["multires_d"] <= F16_MAX_MULTIRES_D))
+        d = _lib.FieldDesc()
+        d.D_density, d.D_color, d.W = c["D_density"], c["D_color"], c["W"]
+        d.geometry_dim, d.color_dim = c["geometry_dim"], c["color_dim"]
+        d.multires_d, d.multires_fg, d.multires_ft, d.multires_view = (c["multires_d"], c["multires_fg"],
+                                                                       c["multires_ft"], c["multires_view"])
+        d.enable_nablas_input = 1 if self.enable_nablas_input else 0
+        return d
+
+    def _fused_problem(self):
+        """None if the fused kernels take this model, otherwise why not.  The input widths and the mesh grid are not in
+        the descriptor and are tested here, first (a CPU or oracle grid never loads the library); the library's
+        ``nmb_field_check`` owns every other limit."""
+        c = self._cfg
+        if c["input_view_dim"] != 3 or c["input_d_dim"] != 1:
+            return "the fused kernels take input_view_dim = 3 and input_d_dim = 1"
+        if not hasattr(getattr(self.mesh_grid, "grid", None), "handle"):
+            return "the mesh grid is not a CUDA neumesh_b200.MeshGrid"
+        if self.mlp_engine not in self._field_check:
+            L = _lib.lib()
+            rc = L.nmb_field_check(C.byref(self._field_desc()), MLP_ENGINES[self.mlp_engine])
+            self._field_check[self.mlp_engine] = L.nmb_last_error().decode() if rc else None
+        return self._field_check[self.mlp_engine]
+
+    def fused_supported(self) -> bool:
+        return self._fused_problem() is None
 
     def indicator_weight_value(self) -> float:
         return float(self.forward_indicator_weight()) if self.learn_indicator_weight else 0.1
@@ -161,12 +154,9 @@ class NeuMesh(nn.Module):
         """``nmb_field`` handle, (re)packed when any parameter, the mesh grid or the engine changed.
         Editors hot-swap ``mesh_grid`` and re-assign ``indicator_vector`` (SURVEY.md section 7.3) - the key below
         covers tensor identity *and* in-place version counters."""
-        if not self.fused_supported():
-            raise RuntimeError("this NeuMesh configuration is outside the fused CUDA kernels' specialisation "
-                               "(W=256, 1-7 layers per MLP, vertex code widths that are multiples of 32 - exactly 32 "
-                               "for the fp32 engine -, non-negative multires, head blocks of at most 64 columns on the "
-                               "tensor-core engines, multires_d <= 16 on the fp16 engine, first layers of at most 256 "
-                               "columns on the fp32 engine)")
+        problem = self._fused_problem()
+        if problem is not None:
+            raise RuntimeError("this NeuMesh configuration is outside the fused CUDA kernels' specialisation: " + problem)
         params = list(self.parameters())
         key = (id(self.mesh_grid), id(self.mesh_grid.grid), self.mlp_engine, float(self.speed_factor),
                tuple((p.data_ptr(), p._version) for p in params))
@@ -174,13 +164,7 @@ class NeuMesh(nn.Module):
             return self._field
         dev = self.geometry_features.device
         _lib.require_cuda(self.geometry_features, "NeuMesh")
-        c = self._cfg
-        d = _lib.FieldDesc()
-        d.D_density, d.D_color, d.W = c["D_density"], c["D_color"], c["W"]
-        d.geometry_dim, d.color_dim = c["geometry_dim"], c["color_dim"]
-        d.multires_d, d.multires_fg, d.multires_ft, d.multires_view = (c["multires_d"], c["multires_fg"],
-                                                                       c["multires_ft"], c["multires_view"])
-        d.enable_nablas_input = 1 if self.enable_nablas_input else 0
+        d = self._field_desc()
         d.indicator_weight = self.indicator_weight_value()
         d.s = float(self.forward_s())
         keep = []

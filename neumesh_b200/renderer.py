@@ -47,22 +47,43 @@ def release_workspace(device: Optional[torch.device] = None) -> None:
             _WORKSPACES.pop(key, None)
 
 
-def fused_eligible(model, rays_o, *, batched, perturb, random_color_direction, use_view_dirs, N_samples, N_importance,
-                   N_upsample_iters, samples_output) -> bool:
-    if torch.is_grad_enabled() or not rays_o.is_cuda:
+def _cascade_eligible(geo, rays_o, *, batched, use_view_dirs, N_samples, N_importance, N_upsample_iters) -> bool:
+    """Whether the fused sampling cascade can serve the geometry model ``geo`` with these arguments: every fused route
+    of ``volume_render`` needs this."""
+    return (isinstance(geo, NeuMesh) and rays_o.is_cuda and geo.geometry_features.is_cuda and geo.fused_supported()
+            and use_view_dirs and (not batched or rays_o.shape[0] == 1) and N_samples >= 2 and N_upsample_iters >= 0
+            and (N_upsample_iters == 0 or N_importance % N_upsample_iters == 0))
+
+
+def fused_eligible(model, rays_o, *, batched, random_color_direction, use_view_dirs, N_samples, N_importance,
+                   N_upsample_iters) -> bool:
+    """Whether ``nmb_render`` renders the whole call: grad mode off, and a ``NeuMesh`` or a texture edit it can render."""
+    if torch.is_grad_enabled() or random_color_direction:
         return False
     if isinstance(model, NeuMesh):
-        if not model.fused_supported() or not model.geometry_features.is_cuda:
-            return False
-    elif not (is_edit_model(model) and getattr(model, "fused_render", True) and edit_fused_supported(model)):
+        geo = model
+    elif is_edit_model(model) and getattr(model, "fused_render", True) and edit_fused_supported(model):
+        geo = model.main_model
+    else:
         return False
-    if random_color_direction or not use_view_dirs:
-        return False
-    if batched and rays_o.shape[0] != 1:
-        return False
-    if N_samples < 2 or N_upsample_iters < 0 or (N_upsample_iters > 0 and N_importance % N_upsample_iters):
-        return False
-    return True
+    return _cascade_eligible(geo, rays_o, batched=batched, use_view_dirs=use_view_dirs, N_samples=N_samples,
+                             N_importance=N_importance, N_upsample_iters=N_upsample_iters)
+
+
+def fused_cascade_model(model, rays_o, *, z_samples, random_color_direction, **cascade_kwargs):
+    """For a call ``nmb_render`` does not render whole: the geometry model whose fused sampling cascade supplies the
+    generic path's sample depths, or None.  Without grad that is the main model of a texture edit (the edit's colour
+    blend then runs per chunk on the generic path); in grad mode a ``NeuMesh`` itself (a training step: the
+    differentiable evaluation at the final samples follows on the generic path)."""
+    if z_samples is not None:
+        return None
+    if torch.is_grad_enabled():
+        geo = model if isinstance(model, NeuMesh) else None
+    elif random_color_direction:
+        return None
+    else:
+        geo = getattr(model, "main_model", None)
+    return geo if _cascade_eligible(geo, rays_o, **cascade_kwargs) else None
 
 
 def render_fused(rays_o, rays_d, model, *, obj_bounding_radius=1.0, calc_normal=False, white_bkgd=False,
@@ -397,9 +418,9 @@ def volume_render(rays_o, rays_d, model, obj_bounding_radius=1.0, batched=False,
     rays_o = torch.reshape(rays_o, flat_shape).float()
     rays_d = torch.reshape(rays_d, flat_shape).float()
 
-    if fused_eligible(model, rays_o, batched=batched, perturb=perturb, random_color_direction=random_color_direction,
-                      use_view_dirs=use_view_dirs, N_samples=N_samples, N_importance=N_importance,
-                      N_upsample_iters=N_upsample_iters, samples_output=samples_output):
+    route = dict(batched=batched, random_color_direction=random_color_direction, use_view_dirs=use_view_dirs,
+                 N_samples=N_samples, N_importance=N_importance, N_upsample_iters=N_upsample_iters)
+    if fused_eligible(model, rays_o, **route):
         out = render_fused(rays_o, rays_d, model, obj_bounding_radius=obj_bounding_radius, calc_normal=calc_normal,
                            white_bkgd=white_bkgd, near_bypass=near_bypass, far_bypass=far_bypass,
                            N_samples=N_samples, N_importance=N_importance, N_upsample_iters=N_upsample_iters,
@@ -410,28 +431,13 @@ def volume_render(rays_o, rays_d, model, obj_bounding_radius=1.0, batched=False,
         return out["rgb"], out["depth_volume"], out
 
     rays_d = F.normalize(rays_d, dim=-1)
-    geo = getattr(model, "main_model", None)   # TextureEditableNeuMesh: geometry (and the cascade) is the main model's
-    if (isinstance(geo, NeuMesh) and not torch.is_grad_enabled() and z_samples is None and rays_o.is_cuda
-            and geo.fused_supported() and geo.geometry_features.is_cuda and use_view_dirs and not random_color_direction
-            and (not batched or rays_o.shape[0] == 1) and N_samples >= 2
-            and (N_upsample_iters == 0 or N_importance % max(N_upsample_iters, 1) == 0)):
-        # texture-edit render (editing/texture_neumesh/texture_renderer.py): fused sampling cascade on the main model's
-        # geometry; the colour blend of the edit runs per live sample through the fused field kernels
-        z_samples = render_fused(rays_o.reshape(-1, 3), rays_d.reshape(-1, 3), geo, obj_bounding_radius=obj_bounding_radius,
-                                 near_bypass=near_bypass, far_bypass=far_bypass, N_samples=N_samples,
-                                 N_importance=N_importance, N_upsample_iters=N_upsample_iters,
-                                 bounded_near_far=bounded_near_far, normalize_dirs=False, min_chunk=rayschunk,
-                                 perturb=perturb, perturb_u=perturb_u, sampling_only=True)["d_all"]
-        if batched:
-            z_samples = z_samples.unsqueeze(0)
-    if (isinstance(model, NeuMesh) and torch.is_grad_enabled() and z_samples is None and rays_o.is_cuda
-            and model.fused_supported() and model.geometry_features.is_cuda and use_view_dirs
-            and (not batched or rays_o.shape[0] == 1) and N_samples >= 2
-            and (N_upsample_iters == 0 or N_importance % max(N_upsample_iters, 1) == 0)):
-        # training step (config 4): the no-grad sampling cascade runs in the fused CUDA kernels; the differentiable
-        # evaluation at the final samples goes through the model protocol below (FusedFieldFn on CUDA)
+    geo = fused_cascade_model(model, rays_o, z_samples=z_samples, **route)
+    if geo is not None:
+        # texture edit (editing/texture_neumesh/texture_renderer.py) or training step (config 4): the no-grad sampling
+        # cascade runs in the fused CUDA kernels; the evaluation at the final samples goes through the model protocol below
+        # (the edit's colour blend per live sample through the fused field kernels, FusedFieldFn in grad mode)
         with torch.no_grad():
-            z_samples = render_fused(rays_o.reshape(-1, 3), rays_d.reshape(-1, 3), model,
+            z_samples = render_fused(rays_o.reshape(-1, 3), rays_d.reshape(-1, 3), geo,
                                      obj_bounding_radius=obj_bounding_radius, near_bypass=near_bypass,
                                      far_bypass=far_bypass, N_samples=N_samples, N_importance=N_importance,
                                      N_upsample_iters=N_upsample_iters, bounded_near_far=bounded_near_far,

@@ -45,6 +45,79 @@ def cuda_model(mesh, cfg, sd, engine="tcgen05", device="cuda:0"):
     return model.to(device).eval()
 
 
+# Configuration matrix of the field engine tests.  Each row exists for the layout property named beside it;
+# test_rows_hit_their_layouts asserts that property from the packing formulas, so that a change of the defaults cannot
+# make a row redundant.
+ROWS = {
+    # default: the geometry head is exactly one fp16 ring step (2 slabs)
+    "A": dict(),
+    # 1-slab geometry head (the fp16 tangent warpgroup pads its only step with a zero slab); raw codes only; one
+    # hidden geometry layer
+    "B": dict(D_density=1, D_color=4, multires_d=4, multires_fg=0, multires_ft=2, multires_view=4,
+              learn_indicator_weight=True),
+    # 3-slab geometry head spanning two fp16 steps (the second shared with a code slab); odd first-layer slab count
+    # (zero padded); deepest geometry net.  multires_d = 16 is the largest the fp16 engine accepts.
+    "C": dict(D_density=7, D_color=2, color_dim=64, multires_d=16, multires_fg=3, multires_ft=1, multires_view=2,
+              learn_indicator_weight=True),
+    # 4-slab geometry head and 64-column colour head (both maxima); 3xTF32 only (multires_d > 16)
+    "D": dict(D_density=3, D_color=3, geometry_dim=64, multires_d=28, multires_fg=2, multires_ft=2, multires_view=0,
+              learn_indicator_weight=True),
+    # 64-column colour head through the view bands; odd code-block counts; one colour layer
+    "E": dict(D_density=2, D_color=1, geometry_dim=96, color_dim=160, multires_d=8, multires_fg=1, multires_ft=0,
+              multires_view=6, learn_indicator_weight=True),
+    # no nabla input; deepest colour net; fixed indicator weight
+    "F": dict(D_density=4, D_color=7, geometry_dim=256, multires_d=6, multires_fg=1, multires_ft=3, multires_view=1,
+              enable_nablas_input=False, learn_indicator_weight=False),
+}
+
+# Configurations just inside and just outside each limit of the fused kernels
+LIMITS = {
+    "colour_head_64": dict(multires_view=6),                    # 17 + 3 + 39 = 59 -> 64 columns
+    "colour_head_80": dict(multires_view=7),                    # 65 -> 80 columns: tensor-core engines refuse
+    "geometry_head_64": dict(multires_d=28, multires_view=0),   # 57 -> 64 (colour head 63 -> 64)
+    "geometry_head_80": dict(multires_d=32, multires_view=0),   # 65 -> 80 (colour head 71 -> 80)
+    "fp16_multires_d_16": dict(multires_d=16, multires_view=2),
+    "fp16_multires_d_17": dict(multires_d=17, multires_view=2),  # tangent seed 2^16 cos: beyond fp16's 65504
+    "fp32_k0_256": dict(multires_fg=3),                         # 32 + 7 * 32 = 256 first-layer columns
+    "fp32_k0_320": dict(multires_fg=4),                         # 320: beyond the fp32 engine's tile
+    "depth_7": dict(D_density=7, D_color=7),
+    "depth_8_geometry": dict(D_density=8),
+    "depth_8_colour": dict(D_color=8),
+}
+EXPECT_INSIDE = {   # engines (f16, tf32, fp32) the library accepts, stated per row
+    "colour_head_64": (1, 1, 1), "colour_head_80": (0, 0, 1), "geometry_head_64": (0, 1, 1),
+    "geometry_head_80": (0, 0, 1), "fp16_multires_d_16": (1, 1, 1), "fp16_multires_d_17": (0, 1, 1),
+    "fp32_k0_256": (1, 1, 1), "fp32_k0_320": (1, 1, 0), "depth_7": (1, 1, 1), "depth_8_geometry": (0, 0, 0),
+    "depth_8_colour": (0, 0, 0),
+}
+
+
+def _a16(n):
+    return (n + 15) // 16 * 16
+
+
+def layout(c):
+    """Head blocks and first-layer slab counts (16 columns each) as csrc/field.cu make_layout packs them."""
+    ch_d = 1 + 2 * c.multires_d
+    off_fg = _a16(ch_d)
+    off_ft = _a16(ch_d + (3 if c.enable_nablas_input else 0) + 3 * (1 + 2 * c.multires_view))
+    k0g = _a16(off_fg + c.geometry_dim * (1 + 2 * c.multires_fg))
+    k0c = _a16(off_ft + c.color_dim * (1 + 2 * c.multires_ft))
+    return dict(head_g=off_fg // 16, head_c=off_ft // 16, slabs_g=k0g // 16, slabs_c=k0c // 16, k0g=k0g, k0c=k0c)
+
+
+def inside(engine, c):
+    """Whether the library accepts configuration c on this engine, written out here from the limits the kernels are
+    built for.  The library states them once (csrc/field.cu check_field, exported as nmb_field_check) and
+    ``NeuMesh.fused_supported()`` asks it; the tests hold the two to each other."""
+    lay = layout(c)
+    if not (1 <= c.D_density <= 7 and 1 <= c.D_color <= 7):
+        return False
+    if engine == "fp32":
+        return c.geometry_dim == 32 and c.color_dim == 32 and lay["k0g"] <= 256 and lay["k0c"] <= 256
+    return lay["head_g"] <= 4 and lay["head_c"] <= 4 and (engine != "tcgen05_f16" or c.multires_d <= 16)
+
+
 def sample_points(n, seed=0):
     g = torch.Generator().manual_seed(seed)
     dirs = torch.nn.functional.normalize(torch.randn(n, 3, generator=g), dim=-1)

@@ -2,6 +2,7 @@
 import ctypes
 import os
 import re
+import types
 
 import numpy as np
 import pytest
@@ -47,14 +48,19 @@ def test_no_cpu_fallback_without_cuda():
         nb.MeshGrid(synth.icosphere_mesh(1), torch.device("cpu"))
 
 
+class _FakeGrid:  # the NeuMesh constructor only needs the vertex count and normals
+    def get_number_of_vertices(self):
+        return 42
+
+    def get_vertex_normal_torch(self):
+        return torch.zeros(42, 3)
+
+
+class _FakeCudaGrid(_FakeGrid):  # passes where only a CUDA MeshGrid's presence is checked (NeuMesh.fused_supported)
+    grid = types.SimpleNamespace(handle=None)
+
+
 def test_state_dict_keys_match_reference():
-    class _FakeGrid:  # constructor only needs the vertex count and normals
-        def get_number_of_vertices(self):
-            return 42
-
-        def get_vertex_normal_torch(self):
-            return torch.zeros(42, 3)
-
     import neumesh_b200 as nb
     cfg = synth.ModelConfig()
     m = nb.NeuMesh(_FakeGrid(), **cfg.model_kwargs())
@@ -66,6 +72,98 @@ def test_state_dict_keys_match_reference():
     cfg2 = synth.ModelConfig(learn_indicator_weight=True)
     m2 = nb.NeuMesh(_FakeGrid(), **cfg2.model_kwargs())
     assert "indicator_weight_raw" in m2.state_dict()
+
+
+def test_fused_supported_asks_the_library():
+    """``fused_supported()`` agrees with the limits the field engine tests state (``helpers.inside``) on every row of
+    their configuration matrix and limit cases, on every engine, on a host without a GPU.  One model per configuration:
+    ``mlp_engine`` is re-assigned between the engines."""
+    import neumesh_b200 as nb
+    engines = ["tcgen05_f16", "tcgen05", "fp32"]
+    for name, kw in list(helpers.ROWS.items()) + list(helpers.LIMITS.items()):
+        cfg = synth.ModelConfig(**kw)
+        m = nb.NeuMesh(_FakeCudaGrid(), **cfg.model_kwargs())
+        for i, engine in enumerate(engines):
+            m.mlp_engine = engine
+            assert m.fused_supported() == helpers.inside(engine, cfg), (name, engine)
+            if name in helpers.EXPECT_INSIDE:
+                assert m.fused_supported() == bool(helpers.EXPECT_INSIDE[name][i]), (name, engine)
+    # what the descriptor does not carry is decided before the library is asked
+    assert not nb.NeuMesh(_FakeGrid(), **synth.ModelConfig().model_kwargs()).fused_supported()
+    assert not nb.NeuMesh(_FakeCudaGrid(), input_view_dim=2, **synth.ModelConfig().model_kwargs()).fused_supported()
+    # the library names the limit; packed_field raises with it before touching a device
+    wide = nb.NeuMesh(_FakeCudaGrid(), **synth.ModelConfig(W=128).model_kwargs())
+    assert not wide.fused_supported()
+    d = wide._field_desc()
+    assert _lib.lib().nmb_field_check(ctypes.byref(d), 2) == 2
+    assert b"W = 256" in _lib.lib().nmb_last_error()
+    with pytest.raises(RuntimeError, match="W = 256"):
+        wide.packed_field()
+
+
+def test_volume_render_routing(monkeypatch):
+    """The fused route ``volume_render`` takes, over models x grad mode x every argument its conditions read.
+    R: ``nmb_render`` renders the whole call (``fused_eligible``); M / S: the fused sampling cascade runs on the edit's
+    main model / on the model itself, the generic path evaluates the samples (``fused_cascade_model``); G: the generic
+    path throughout.  Stand-ins replace the CUDA tensors; the expected routes are written out by hand."""
+    import neumesh_b200 as nb
+    cuda = types.SimpleNamespace(is_cuda=True)
+
+    def neumesh(cuda_tables, W=256):
+        m = nb.NeuMesh(_FakeCudaGrid(), **synth.ModelConfig(W=W).model_kwargs())
+        if cuda_tables:
+            m.__dict__["geometry_features"] = cuda   # shadows the CPU parameter where .is_cuda is read
+        return m
+
+    class Edit:   # the attributes of a texture-edit model; `eligible` stands for what edit_fused_supported checks
+        def __init__(self, main, eligible=True, fused_render=True):
+            self.main_model, self.ref_models = main, [main]
+            self.main_editing_masks = self.main_editing_colorfeats = self.rot_s_m = None
+            self.eligible, self.fused_render = eligible, fused_render
+
+    monkeypatch.setattr(nbr, "edit_fused_supported", lambda m: m.eligible and m.main_model.geometry_features.is_cuda)
+
+    def models(cuda_tables=True):
+        # NeuMesh, NeuMesh with W = 128, eligible edit, ineligible edit, edit with fused_render = False, foreign model
+        return [neumesh(cuda_tables), neumesh(cuda_tables, W=128), Edit(neumesh(cuda_tables)),
+                Edit(neumesh(cuda_tables), eligible=False), Edit(neumesh(cuda_tables), fused_render=False),
+                torch.nn.Linear(1, 1)]
+
+    def rays(batch=None, on_cuda=True):
+        return types.SimpleNamespace(is_cuda=on_cuda, shape=(4, 3) if batch is None else (batch, 4, 3))
+
+    # name: (keyword changes, routes of the six models without grad, routes in grad mode)
+    table = {
+        "defaults": (dict(), "RGRMMG", "SGGGGG"),
+        "random_color_direction": (dict(random_color_direction=True), "GGGGGG", "SGGGGG"),
+        "no view dirs": (dict(use_view_dirs=False), "GGGGGG", "GGGGGG"),
+        "batched, B = 1": (dict(batched=True, rays_o=rays(1)), "RGRMMG", "SGGGGG"),
+        "batched, B = 2": (dict(batched=True, rays_o=rays(2)), "GGGGGG", "GGGGGG"),
+        "N_samples = 2": (dict(N_samples=2), "RGRMMG", "SGGGGG"),
+        "N_samples = 1": (dict(N_samples=1), "GGGGGG", "GGGGGG"),
+        "no up-sampling": (dict(N_upsample_iters=0), "RGRMMG", "SGGGGG"),
+        "N_importance not divisible": (dict(N_upsample_iters=3), "GGGGGG", "GGGGGG"),
+        # nmb_render rejects a negative count, so neither fused route may take it
+        "N_upsample_iters < 0": (dict(N_upsample_iters=-1), "GGGGGG", "GGGGGG"),
+        "z_samples given": (dict(z_samples=torch.zeros(4, 128)), "RGRGGG", "GGGGGG"),
+        "rays on the CPU": (dict(rays_o=rays(on_cuda=False)), "GGGGGG", "GGGGGG"),
+        "tables on the CPU": (dict(cuda_tables=False), "GGGGGG", "GGGGGG"),
+    }
+    for name, (change, want_nograd, want_grad) in table.items():
+        kw = dict(rays_o=rays(), batched=False, random_color_direction=False, use_view_dirs=True, N_samples=64,
+                  N_importance=64, N_upsample_iters=4, z_samples=None, cuda_tables=True)
+        kw.update(change)
+        rays_o, z_samples, ms = kw.pop("rays_o"), kw.pop("z_samples"), models(kw.pop("cuda_tables"))
+        for grad, want in ((False, want_nograd), (True, want_grad)):
+            got = ""
+            for m in ms:
+                with torch.set_grad_enabled(grad):
+                    if nbr.fused_eligible(m, rays_o, **kw):
+                        got += "R"
+                        continue
+                    geo = nbr.fused_cascade_model(m, rays_o, z_samples=z_samples, **kw)
+                got += "G" if geo is None else "S" if geo is m else "M" if geo is m.main_model else "?"
+            assert got == want, (name, "grad" if grad else "no grad", got, want)
 
 
 def test_generic_renderer_path_equals_oracle(golden_dir):

@@ -423,9 +423,8 @@ def test_edit_eligibility_cpu():
     assert not tn.is_edit_model(main)
     # a CPU edit model is never fused
     assert not tn.edit_fused_supported(model)
-    assert not R.fused_eligible(model, torch.zeros(4, 3), batched=False, perturb=False, random_color_direction=False,
-                                use_view_dirs=True, N_samples=64, N_importance=64, N_upsample_iters=4,
-                                samples_output=False)
+    assert not R.fused_eligible(model, torch.zeros(4, 3), batched=False, random_color_direction=False,
+                                use_view_dirs=True, N_samples=64, N_importance=64, N_upsample_iters=4)
     with pytest.raises(ValueError, match="fused kernels"):
         tn.packed_edit(model)
     # shape errors are reported before anything touches a device
