@@ -34,6 +34,9 @@ const char* nmb_last_error(void);
 int nmb_version(void);
 /* number of kernels this library has launched in the calling process since load (bench.py: gpu_launches) */
 int64_t nmb_launch_count(void);
+/* number of device buffers (cudaMalloc) the library's handles have allocated in the calling process since load; stream-
+ * ordered scratch taken from the device's memory pool is not counted */
+int64_t nmb_alloc_count(void);
 
 /* Per-kernel-class device timing for roofline reports (bench.py): when enabled, CUDA events are recorded on the
  * launching stream around every launch of a class; collect() synchronises those events and returns, per class
@@ -48,6 +51,16 @@ int nmb_profile_collect(double* ms, int64_t* launches, int64_t* units, int n_cla
  * whose only kept result is the `grid` tuple).  Builds a Morton-ordered sparse octree with tight node boxes.
  * Synchronises the stream (build is a one-off per mesh). */
 int nmb_grid_create(const float* vertices /*[V,3]*/, int64_t V, void* stream, nmb_grid** out);
+/* Rebuild the octree of `g` over moved vertices (a deformation: editing/render_geometry_editing.py:37-67 builds a new
+ * MeshGrid instead).  V must equal the grid's vertex count.  The result is what nmb_grid_create gives on the same
+ * vertices (same nmb_grid_order, same neighbours); the grid's device buffers are reused, so repeated updates allocate
+ * nothing once the node array has settled.  Every call that passes the V check increments the grid's generation, a
+ * failed one too (the grid must then be updated again before use).  Fields and edits packed before are refused by
+ * every call that reads them until nmb_field_update / nmb_edit_update re-pack them into the new slot order.  The caller
+ * makes sure no work that reads the grid is in flight on another stream.  Synchronises the stream. */
+int nmb_grid_update(nmb_grid* g, const float* vertices /*[V,3]*/, int64_t V, void* stream);
+/* number of nmb_grid_update calls on this grid (0 after nmb_grid_create) */
+int64_t nmb_grid_generation(const nmb_grid* g);
 void nmb_grid_destroy(nmb_grid* g);
 int64_t nmb_grid_num_vertices(const nmb_grid* g);
 /* sorted slot -> original vertex index, int32 [V] (device pointer owned by the grid) */
@@ -96,7 +109,9 @@ typedef struct nmb_field_desc {
  * 2 = wgmma fp16x3 tensor-core MLP (fp16 hi/lo operands, weights packed as 2^8 W; the Python layer's default engine) */
 int nmb_field_create(const nmb_grid* g, const nmb_field_desc* desc, int mlp_engine, void* stream, nmb_field** out);
 void nmb_field_destroy(nmb_field* f);
-/* re-pack after the caller changed parameter values in place (same shapes) */
+/* re-pack after the caller changed parameter values in place (same shapes), or after nmb_grid_update moved the grid's
+ * vertices: the vertex tables are permuted into the grid's current slot order and the shell certificate is dropped (it
+ * is rebuilt by the next call that needs it).  Same-size buffers are reused. */
 int nmb_field_update(nmb_field* f, const nmb_field_desc* desc, void* stream);
 /* Whether the fused kernels take this configuration on this engine: 0, or 2 with the reason in nmb_last_error().
  * Reads only the integer fields of desc (no pointer is dereferenced) and makes no CUDA call, so it also answers on a host
@@ -197,7 +212,8 @@ typedef struct nmb_edit nmb_edit;
 int nmb_edit_create(const nmb_field* main_field, int32_t n_ref, const nmb_field* const* ref_fields,
                     const uint8_t* masks, const float* codes, int64_t V, int32_t color_dim,
                     const float* rotations_host, void* stream, nmb_edit** out);
-/* new values for masks, codes and rotations (same shapes as at creation) */
+/* new values for masks, codes and rotations (same shapes as at creation); also the re-pack after nmb_grid_update moved
+ * the main grid's vertices (an edit packed before is refused by nmb_render_edit until then) */
 int nmb_edit_update(nmb_edit* e, const uint8_t* masks, const float* codes, const float* rotations_host, void* stream);
 void nmb_edit_destroy(nmb_edit* e);
 /* bytes of scratch nmb_render_edit needs for `rays_per_chunk` rays (== nmb_render_workspace_bytes when edit is NULL) */
@@ -239,6 +255,14 @@ int nmb_pack_bgr8(const float* rgb, int64_t N, uint8_t* bgr8, void* stream);
  * normals must be rebuilt (editing/render_geometry_editing.py:37-67). */
 int nmb_vertex_normals(const float* vertices, int64_t V, const int32_t* triangles, int64_t T, float* normals,
                        void* stream);
+
+/* deform_model's indicator rotation (editing/render_geometry_editing.py:44-65), one thread per vertex in fp32:
+ * axis = cross(n_old, n_new); c = clamp(dot / (|n_old| |n_new|), -1, 1); aa = axis * acos(c) (so |aa| = theta |axis|,
+ * as the reference computes it); R = kornia's angle_axis_to_rotation_matrix(aa) (Rodrigues with w = aa / (|aa| + 1e-6)
+ * where aa.aa > 1e-6, I + [aa]x otherwise); ind_out = R ind, negated where c == -1.  Formula, operation order and
+ * hand-checked cases: oracle/deform.py.  n_old, n_new, ind_in, ind_out [V,3]; ind_out may alias ind_in. */
+int nmb_indicator_rotate(const float* n_old, const float* n_new, const float* ind_in, int64_t V, float* ind_out,
+                         void* stream);
 
 /* ---- training-path primitives (config 4: forward + backward through the field) -----------------------------------
  * The reference trains through the renderer with autograd: models/trainer.py:75-80 (forward), :173-262 (losses on rgb,

@@ -8,6 +8,7 @@ Public surface (mirrors the reference's Python API for this path):
 * ``volume_render`` / ``SingleRenderer`` <- models/renderer.py
 * ``TextureEditableNeuMesh`` <- editing/texture_neumesh/texture_neumesh.py
 * ``parallel.render_sharded`` <- the ``nn.DataParallel`` ray scatter / gather of models/trainer.py:39-42
+* ``deform_model``      <- editing/render_geometry_editing.py:37-67 (also in place, from a CUDA tensor of vertices)
 
 The compute lives in ``lib/libneumesh_b200.so`` (hand-written sm_90a CUDA behind the C ABI of
 ``include/neumesh_b200.h``); importing this package does not load it, using it does - and fails loudly if the
@@ -18,8 +19,9 @@ from .neumesh import Embedder, NeuMesh, get_embedder, interpolation  # noqa: F40
 from .renderer import SingleRenderer, release_workspace, volume_render  # noqa: F401
 from .texture_neumesh import TextureEditableNeuMesh  # noqa: F401
 from .neus import NeuS  # noqa: F401
+from .deform import deform_model, indicator_rotate  # noqa: F401
 from . import parallel  # noqa: F401
 
 __all__ = ["NeuMesh", "MeshGrid", "MeshPrimitive", "GridHandle", "frnn_grid_points", "volume_render",
            "release_workspace", "TextureEditableNeuMesh", "SingleRenderer", "Embedder", "get_embedder",
-           "interpolation", "parallel", "NeuS"]
+           "interpolation", "parallel", "NeuS", "deform_model", "indicator_rotate"]

@@ -50,9 +50,12 @@ SIGNATURES = {
     "nmb_last_error": (C.c_char_p, []),
     "nmb_version": (C.c_int, []),
     "nmb_launch_count": (_I64, []),
+    "nmb_alloc_count": (_I64, []),
     "nmb_profile_enable": (None, [C.c_int]),
     "nmb_profile_collect": (C.c_int, [C.POINTER(C.c_double), C.POINTER(_I64), C.POINTER(_I64), C.c_int]),
     "nmb_grid_create": (C.c_int, [_P, _I64, _P, C.POINTER(_P)]),
+    "nmb_grid_update": (C.c_int, [_P, _P, _I64, _P]),
+    "nmb_grid_generation": (_I64, [_P]),
     "nmb_grid_destroy": (None, [_P]),
     "nmb_grid_num_vertices": (_I64, [_P]),
     "nmb_grid_order": (_P, [_P]),
@@ -80,6 +83,7 @@ SIGNATURES = {
     "nmb_first_crossing": (C.c_int, [_P, _I64, _I32, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "nmb_pack_bgr8": (C.c_int, [_P, _I64, _P, _P]),
     "nmb_vertex_normals": (C.c_int, [_P, _I64, _P, _I64, _P, _P]),
+    "nmb_indicator_rotate": (C.c_int, [_P, _P, _P, _I64, _P, _P]),
     "nmb_get_rays": (C.c_int, [C.POINTER(_F), C.POINTER(_F), _I32, _I32, _P, _P, _P]),
     # training-path primitives (csrc/train.cu); the nmb_tr_inputs struct is bound in train_ops.TrInputs
     "nmb_tr_gemm": (C.c_int, [_P, _I64, C.c_int, _P, _I64, C.c_int, _P, _I64, _I64, _I64, _I64, _P, C.c_int, _P, _I64,
@@ -137,6 +141,11 @@ def require_cuda(t: torch.Tensor, what: str):
 
 def launch_count() -> int:
     return int(lib().nmb_launch_count())
+
+
+def alloc_count() -> int:
+    """Device buffers the library's handles have allocated in this process (``nmb_alloc_count``)."""
+    return int(lib().nmb_alloc_count())
 
 
 PROFILE_CLASSES = ("knn", "bound_scan", "geo", "geo_jvp", "color", "sampler", "knn_list")

@@ -9,8 +9,10 @@
 namespace nmb {
 static thread_local std::string g_error;
 static std::atomic<int64_t> g_launches{0};
+static std::atomic<int64_t> g_allocs{0};
 void set_error(const std::string& msg) { g_error = msg; }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+void count_alloc() { g_allocs.fetch_add(1, std::memory_order_relaxed); }
 int sm_count() {
   static std::atomic<int> cached[NMB_MAX_DEVICES];   // per device of this process; 0 = not queried yet
   int dev = 0;
@@ -106,4 +108,5 @@ int nmb_profile_collect(double* ms, int64_t* launches, int64_t* units, int n_tag
 const char* nmb_last_error(void) { return nmb::g_error.c_str(); }
 int nmb_version(void) { return NMB_VERSION; }
 int64_t nmb_launch_count(void) { return nmb::g_launches.load(); }
+int64_t nmb_alloc_count(void) { return nmb::g_allocs.load(); }
 }

@@ -10,6 +10,7 @@ namespace nmb {
 
 void set_error(const std::string& msg);
 void count_launch(int n = 1);
+void count_alloc();   // one cudaMalloc by a DevBuf (nmb_alloc_count)
 
 #define NMB_CUDA_OK(expr)                                                                               \
   do {                                                                                                  \
@@ -143,7 +144,14 @@ struct DevBuf {
     release();
     n = count;
     if (count <= 0) return cudaSuccess;
+    count_alloc();
     return cudaMalloc(reinterpret_cast<void**>(&p), sizeof(T) * static_cast<size_t>(count));
+  }
+  // at least `count` elements: a buffer that is already large enough is kept (n stays its capacity); otherwise
+  // `count + count * headroom_pct / 100` are allocated, so that a slowly varying size settles after one reallocation
+  cudaError_t reserve(int64_t count, int headroom_pct = 0) {
+    if (p && n >= count) return cudaSuccess;
+    return alloc(count + count * headroom_pct / 100);
   }
   void release() {
     if (p) cudaFree(p);

@@ -18,6 +18,7 @@
 struct nmb_edit {
   const nmb_field* main = nullptr;
   const nmb_grid* grid = nullptr;
+  int64_t grid_generation = 0;  // grid->generation the masks and codes were permuted for
   int n_ref = 0;
   int Fc = 0;
   std::vector<const nmb_field*> refs;
@@ -157,6 +158,7 @@ int upload(nmb_edit* e, const uint8_t* masks, const float* codes, const float* r
   e->has_rot = rotations != nullptr;
   e->rot.assign(rotations ? rotations : nullptr, rotations ? rotations + 9 * e->n_ref : nullptr);
   NMB_CUDA_OK(cudaStreamSynchronize(stream));   // the caller may free or overwrite its inputs when this returns
+  e->grid_generation = e->grid->generation;
   return 0;
 }
 
@@ -195,6 +197,8 @@ bool edit_needs_nabla(const nmb_edit* e) {
 }
 
 const nmb_grid* edit_grid(const nmb_edit* e) { return e->grid; }
+
+bool edit_fresh(const nmb_edit* e) { return e->grid_generation == e->grid->generation; }
 
 int apply_edit(const nmb_edit* e, const FieldIn& in, int64_t n, float* rgb, const EditScratch& s, cudaStream_t stream) {
   if (n <= 0) return 0;

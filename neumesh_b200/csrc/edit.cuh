@@ -34,6 +34,9 @@ bool edit_needs_nabla(const nmb_edit* e);
 // the main grid the edit's masks and codes are permuted to
 const nmb_grid* edit_grid(const nmb_edit* e);
 
+// false if that grid was updated (nmb_grid_update) after the edit's tables were permuted to its slot order
+bool edit_fresh(const nmb_edit* e);
+
 // Blend the references of `e` into rgb ([3][in.stride] SoA, the main colour of the n points described by `in`:
 // ds, slot, w, nabla (nullable unless a reference takes nabla), dirs or rays_d / R).  Reads one count back per
 // reference (synchronises the stream).

@@ -155,8 +155,10 @@ static int pack_field(const nmb_field_desc* d, nmb_field* f, cudaStream_t stream
   int rc = check_field(d, f->engine);
   if (rc) return rc;
   f->lay = make_layout(d);
+  // the certificate depends on the vertex positions and the indicator: rebuilt lazily for the tables packed below
   f->shell_valid = false;
   f->shell = ShellGrid{};
+  f->grid_generation = g->generation;
   f->w1 = d->indicator_weight;
   f->s = d->s;
   NMB_CUDA_OK(f->indicator.alloc(g->V));
@@ -243,6 +245,7 @@ static int field_query(const nmb_field* f, const float* xyz, const float* dirs, 
                        int64_t* idx_out = nullptr, float* w_out = nullptr) {
   using namespace nmb;
   NMB_CHECK(f != nullptr, "null field");
+  NMB_CHECK_FRESH(f);
   if (M <= 0) return 0;
   const bool need_nabla = (nabla != nullptr) || (want_color && f->lay.use_nabla);
   // scratch: ds 1, slot 8, w 8, grad 3, nabla 3, rgb 3, sdf 1 = 27 words per point
@@ -285,6 +288,7 @@ static int field_query(const nmb_field* f, const float* xyz, const float* dirs, 
 
 int nmb_field_shell_grid(const nmb_field* f, uint8_t* cells, int32_t* G, float* B, void* stream_) {
   NMB_CHECK(f != nullptr && G != nullptr && B != nullptr, "null argument");
+  NMB_CHECK_FRESH(f);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   int rc = nmb::ensure_shell_grid(f, stream);
   if (rc) return rc;
@@ -319,6 +323,7 @@ int nmb_field_color(const nmb_field* f, const float* color_table, int64_t table_
                     void* stream_) {
   using namespace nmb;
   NMB_CHECK(f != nullptr && ds && idx && w && view_dirs && rgb, "null argument");
+  NMB_CHECK_FRESH(f);
   NMB_CHECK(!f->lay.use_nabla || nabla != nullptr, "this field's colour network takes nabla as an input");
   NMB_CHECK(color_table == nullptr || table_rows > 0, "table_rows must be positive when a table is given");
   if (M <= 0) return 0;

@@ -48,6 +48,7 @@ struct MlpTc {              // tensor-core engine: per layer, per 16-column K-sl
 
 struct nmb_field {
   const nmb_grid* grid = nullptr;
+  int64_t grid_generation = 0;    // grid->generation the vertex tables were permuted for (stale when behind)
   int engine = 0;
   nmb::FieldLayout lay{};
   float w1 = 0.1f, s = 1.f;
@@ -98,6 +99,12 @@ inline int launch_geo(const nmb_field* f, const FieldIn& in, int64_t P, float* s
 inline int launch_color(const nmb_field* f, const FieldIn& in, int64_t P, float* rgb, cudaStream_t s) {
   return f->engine != 1 ? launch_color_tc(f, in, P, rgb, s) : launch_color_ffma(f, in, P, rgb, s);
 }
+
+// refuses a field packed before its grid's last nmb_grid_update (its tables are in the old slot order)
+#define NMB_CHECK_FRESH(f)                                                                                          \
+  NMB_CHECK((f)->grid_generation == (f)->grid->generation,                                                          \
+            "the field was packed before its mesh grid was last updated (nmb_grid_update): re-pack it with "         \
+            "nmb_field_update")
 
 int permute_indicator(const nmb_grid* g, const float* indicator, float4* dst, cudaStream_t stream);
 int pack_mlp_tc(const nmb_field_desc* d, const FieldLayout& lay, nmb_field* f, cudaStream_t stream);

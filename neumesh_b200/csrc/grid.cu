@@ -359,7 +359,10 @@ static int build_grid(const float* vertices, int64_t V, cudaStream_t stream, nmb
   }
   g->num_nodes = n_nodes;
   g->lvl_off = lvl_off;
-  NMB_CUDA_OK(g->nodes.alloc(NODE_F4 * (int64_t)n_nodes));
+  // a rebuild over moved vertices (nmb_grid_update) keeps the node array while it has 1/8 to spare: the node count
+  // varies a little from one deformation to the next, so the array settles after the first update
+  const int64_t node_f4 = NODE_F4 * (int64_t)n_nodes;
+  NMB_CUDA_OK(g->nodes.p ? g->nodes.reserve(node_f4 + node_f4 / 8, 12) : g->nodes.alloc(node_f4));
   for (int l = (int)lvl_off.size() - 2; l >= 0; --l) {
     const int32_t first = lvl_off[l], cnt = lvl_off[l + 1] - lvl_off[l];
     if (cnt <= 0) continue;
@@ -850,6 +853,17 @@ int nmb_grid_create(const float* vertices, int64_t V, void* stream, nmb_grid** o
   *out = g;
   return 0;
 }
+
+int nmb_grid_update(nmb_grid* g, const float* vertices, int64_t V, void* stream) {
+  NMB_CHECK(g != nullptr && vertices != nullptr, "null grid / vertices");
+  NMB_CHECK(V == g->V, "nmb_grid_update keeps the vertex count: V must equal the grid's");
+  // the same build as nmb_grid_create, into the grid's own buffers (all of size V except the node array)
+  int rc = nmb::build_grid(vertices, V, static_cast<cudaStream_t>(stream), g);
+  ++g->generation;   // after a failure too: the tables may be half rebuilt, so nothing packed before may read them
+  return rc;
+}
+
+int64_t nmb_grid_generation(const nmb_grid* g) { return g ? g->generation : 0; }
 
 void nmb_grid_destroy(nmb_grid* g) { delete g; }
 

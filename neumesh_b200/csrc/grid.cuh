@@ -8,6 +8,9 @@ struct nmb_grid {
   int64_t V = 0;
   int levels = 0;          // octree depth L (codes have 3*L bits)
   int num_nodes = 0;
+  // incremented by every nmb_grid_update: fields and edits record the value they were packed against (their vertex
+  // tables are in this grid's slot order, which an update changes) and are refused while it is behind
+  int64_t generation = 0;
   float bmin[3] = {0, 0, 0};
   float inv_cell = 0.f;    // 2^L / cube side
   nmb::DevBuf<float4> pts;     // [V] sorted by Morton code: x, y, z, __int_as_float(original index)

@@ -626,7 +626,11 @@ static int render_impl(const nmb_field* f, const nmb_edit* edit, const nmb_rende
   using namespace nmb;
   if (N <= 0) return 0;   // an empty shard: nothing to do (the output pointers of empty tensors are null)
   NMB_CHECK(f && cfg && rays_o && rays_d, "null argument");
+  NMB_CHECK_FRESH(f);
   NMB_CHECK(!edit || edit_grid(edit) == f->grid, "the edit was created for another main model's mesh grid");
+  NMB_CHECK(!edit || edit_fresh(edit),
+            "the edit was packed before its main mesh grid was last updated (nmb_grid_update): re-pack it with "
+            "nmb_edit_update");
   NMB_CHECK(!edit || !cfg->sampling_only, "an edit changes colour only: sampling_only renders take nmb_render");
   NMB_CHECK(cfg->sampling_only ? (detail != nullptr) : (rgb && depth && acc), "null output");
   NMB_CHECK(rays_per_chunk > 0, "rays_per_chunk must be positive");

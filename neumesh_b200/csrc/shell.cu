@@ -183,7 +183,10 @@ int ensure_shell_grid(const nmb_field* f, cudaStream_t stream) {
   f->shell = ShellGrid{};
   f->shell_valid = true;   // whatever happens below, do not retry on every frame
   if (g->lvl_off.size() < 2 || !(f->w1 > 0.f)) return 0;
-  NMB_CUDA_OK(f->node_normals.alloc(g->num_nodes));
+  // the node count changes when the grid is rebuilt over moved vertices (nmb_grid_update): keep 1/8 to spare then, as
+  // the grid does for its node array
+  const int64_t nn = g->num_nodes;
+  NMB_CUDA_OK(g->generation > 0 ? f->node_normals.reserve(nn + nn / 8, 12) : f->node_normals.alloc(nn));
   NMB_CUDA_OK(f->shell_cells.alloc((int64_t)SHELL_G * SHELL_G * SHELL_G));
   for (int l = (int)g->lvl_off.size() - 2; l >= 0; --l) {
     const int32_t first = g->lvl_off[l], cnt = g->lvl_off[l + 1] - g->lvl_off[l];

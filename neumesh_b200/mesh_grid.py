@@ -27,6 +27,24 @@ class GridHandle:
         self.handle = h
         self.num_vertices = int(self.vertices.shape[0])
 
+    def update(self, vertices: torch.Tensor):
+        """``nmb_grid_update``: rebuild the octree over moved vertices (same count), reusing the grid's buffers.
+        ``self.vertices`` takes the new positions in place; fields and edits packed before must be re-packed."""
+        _lib.require_cuda(vertices, "GridHandle.update")
+        if tuple(vertices.shape) != (self.num_vertices, 3):
+            raise ValueError("GridHandle.update keeps the vertex count: expected [%d, 3], got %s"
+                             % (self.num_vertices, tuple(vertices.shape)))
+        if vertices.data_ptr() != self.vertices.data_ptr():
+            self.vertices.copy_(vertices.detach())
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().nmb_grid_update(self.handle, _lib.ptr(self.vertices), self.num_vertices,
+                                                  _lib.stream_ptr(self.device)))
+
+    @property
+    def generation(self) -> int:
+        """Number of ``update`` calls so far (``nmb_grid_generation``): part of the packed fields' cache keys."""
+        return int(_lib.lib().nmb_grid_generation(self.handle))
+
     def __del__(self):
         h, self.handle = getattr(self, "handle", None), None
         if h:
@@ -133,6 +151,26 @@ class MeshGrid(MeshPrimitive):
         mid = (ind[idx] * w1 + v * rho) / (w1 + rho)
         ds = (w.unsqueeze(-1) * (v * mid).sum(dim=-1, keepdim=True)).sum(dim=-2)
         return ds, idx, w
+
+    def deform_(self, vertices, normals=None):
+        """Move the mesh's vertices in place: ``vertices`` is a CUDA ``[V,3]`` tensor with the grid's vertex count.
+        ``self.vertices`` is overwritten, the octree rebuilt in its buffers (``nmb_grid_update``), and
+        ``vertex_normals`` becomes ``normals`` or, without them, the area-weighted normals of the moved mesh
+        (``nmb_vertex_normals`` over ``mesh.triangles``, uploaded on the first call).  The previous ``vertex_normals``
+        tensor is replaced, not overwritten, so a caller holding it keeps the old normals."""
+        from .renderer import vertex_normals
+        _lib.require_cuda(vertices, "MeshGrid.deform_")
+        self.grid.update(vertices)   # checks the shape, copies into self.vertices (the grid's own tensor)
+        if normals is None:
+            if getattr(self, "_triangles", None) is None:
+                tri = getattr(self.mesh, "triangles", None)
+                if tri is None:
+                    raise ValueError("MeshGrid.deform_ without normals needs mesh.triangles to compute them")
+                self._triangles = torch.as_tensor(np.asarray(tri), dtype=torch.int32).to(self.vertices.device)
+            normals = vertex_normals(self.vertices, self._triangles)
+        elif tuple(normals.shape) != tuple(self.vertices.shape):
+            raise ValueError("normals must be [V,3] like the vertices, got %s" % (tuple(normals.shape),))
+        self.vertex_normals = normals.detach().to(self.vertices.device, torch.float32).contiguous()
 
     def get_vertex_normal_torch(self):
         return self.vertex_normals

@@ -153,13 +153,14 @@ class NeuMesh(nn.Module):
     def packed_field(self):
         """``nmb_field`` handle, (re)packed when any parameter, the mesh grid or the engine changed.
         Editors hot-swap ``mesh_grid`` and re-assign ``indicator_vector`` (SURVEY.md section 7.3) - the key below
-        covers tensor identity *and* in-place version counters."""
+        covers tensor identity *and* in-place version counters.  A grid deformed in place (``MeshGrid.deform_``) has a
+        new generation: the same handle is re-packed (``nmb_field_update``) into the grid's new slot order."""
         problem = self._fused_problem()
         if problem is not None:
             raise RuntimeError("this NeuMesh configuration is outside the fused CUDA kernels' specialisation: " + problem)
         params = list(self.parameters())
-        key = (id(self.mesh_grid), id(self.mesh_grid.grid), self.mlp_engine, float(self.speed_factor),
-               tuple((p.data_ptr(), p._version) for p in params))
+        key = (id(self.mesh_grid), id(self.mesh_grid.grid), self.mlp_engine, self.mesh_grid.grid.generation,
+               float(self.speed_factor), tuple((p.data_ptr(), p._version) for p in params))
         if self._field is not None and key == self._field_key:
             return self._field
         dev = self.geometry_features.device

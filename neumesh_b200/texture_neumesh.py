@@ -84,7 +84,8 @@ def _tensor_key(t):
 
 def packed_edit(model):
     """``nmb_edit`` handle of a texture-edit model, cached per model and rebuilt when a field handle, the masks, the
-    codes or the rotations changed (tensor identity and in-place version counters, as ``NeuMesh.packed_field``)."""
+    codes or the rotations changed (tensor identity and in-place version counters, as ``NeuMesh.packed_field``), or the
+    main model's grid was deformed in place (its generation: the masks and codes are re-permuted by ``nmb_edit_update``)."""
     problem = _edit_problem(model)
     if problem is not None:
         raise ValueError("neumesh_b200: cannot render this texture edit on the fused path: " + problem)
@@ -93,7 +94,7 @@ def packed_edit(model):
     fields = [main.packed_field()] + [r.packed_field() for r in refs]
     # the handle objects themselves (kept alive by the cache entry): a re-created field is a new object
     key_fields = tuple(id(h) for h in fields)
-    key_vals = (_tensor_key(masks), _tensor_key(codes), _tensor_key(rot))
+    key_vals = (_tensor_key(masks), _tensor_key(codes), _tensor_key(rot), main.mesh_grid.grid.generation)
     entry = _EDITS.get(model)
     if entry is not None and entry.key == (key_fields, key_vals):
         return entry.handle
