@@ -113,6 +113,8 @@ def inside(engine, c):
     lay = layout(c)
     if not (1 <= c.D_density <= 7 and 1 <= c.D_color <= 7):
         return False
+    if not all(n >= 32 and n % 32 == 0 for n in (c.geometry_dim, c.color_dim)):   # vertex codes in 32-column blocks
+        return False
     if engine == "fp32":
         return c.geometry_dim == 32 and c.color_dim == 32 and lay["k0g"] <= 256 and lay["k0c"] <= 256
     return lay["head_g"] <= 4 and lay["head_c"] <= 4 and (engine != "tcgen05_f16" or c.multires_d <= 16)
