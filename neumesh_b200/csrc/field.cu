@@ -260,12 +260,7 @@ static int field_query(const nmb_field* f, const float* xyz, const float* dirs, 
     rc = launch_export_knn(f->grid, ko, M, ds_out, idx_out, w_out, nullptr, stream);
     if (rc) return rc;
   }
-  FieldIn in{};
-  in.ds = ko.ds;
-  in.slot = ko.slot;
-  in.w = ko.w;
-  in.grad = ko.grad;
-  in.stride = M;
+  FieldIn in(ko);
   float* nab = sc + 20 * M;
   float* rgb_soa = sc + 23 * M;
   float* sdf_tmp = sdf ? sdf : sc + 26 * M;

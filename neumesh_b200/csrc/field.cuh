@@ -69,6 +69,11 @@ namespace nmb {
 
 // Inputs of a field evaluation over P points whose neighbours are known (SoA from the KNN kernel).
 struct FieldIn {
+  FieldIn() = default;
+  // the neighbours a KNN kernel found; every other member null
+  explicit FieldIn(const KnnOut& k)
+      : ds(k.ds), slot(k.slot), w(k.w), grad(k.grad), stride(k.stride), nabla(nullptr), dirs(nullptr), rays_d(nullptr),
+        R(0), color_table(nullptr), index(nullptr) {}
   const float* ds;        // [P]
   const int32_t* slot;    // [8][P]
   const float* w;         // [8][P]

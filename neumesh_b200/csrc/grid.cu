@@ -27,14 +27,6 @@ namespace nmb {
 // ------------------------------------------------------------------------------------------------------------
 // build
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t expand_bits10(uint32_t v) {
-  v = (v * 0x00010001u) & 0xFF0000FFu;
-  v = (v * 0x00000101u) & 0x0F00F00Fu;
-  v = (v * 0x00000011u) & 0xC30C30C3u;
-  v = (v * 0x00000005u) & 0x49249249u;
-  return v;
-}
-
 __global__ void bbox_kernel(const float* __restrict__ v, int64_t V, float* __restrict__ out /*6: min xyz, max xyz*/) {
   float lo[3] = {CUDART_INF_F, CUDART_INF_F, CUDART_INF_F};
   float hi[3] = {-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F};
@@ -545,8 +537,6 @@ int launch_knn_lists(const nmb_grid* g, const float4* indicator_sorted, float w1
   NMB_LAUNCH_OK();
   return 0;
 }
-
-constexpr int64_t RAY_KERNEL_MIN_RAYS = 32768;  // below this the per-point kernels expose more parallelism
 
 int launch_knn_distance(const nmb_grid* g, const float4* indicator_sorted, float w1, PointSrc src, int64_t P,
                         KnnOut out, cudaStream_t stream) {

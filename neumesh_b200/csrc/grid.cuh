@@ -27,6 +27,18 @@ constexpr int LEAF_MAX = 32;      // nodes with <= LEAF_MAX points are leaves (m
 constexpr int NODE_F4 = 4;        // float4 per node: {lo, link}, {hi, count}, {centre, r}, {axis, t}
 constexpr int DISC_MAX_POINTS = 8192;  // nodes larger than this get the trivial disc (sphere) bound
 constexpr int STACK_MAX = 96;     // traversal stack entries (7 * depth + 8 <= 78 for depth 10)
+// from this many rays on, one thread per ray (or ray segment) fills the GPU; below it the per-point kernels expose more
+// parallelism
+constexpr int64_t RAY_KERNEL_MIN_RAYS = 32768;
+
+// the 10 bits of v spread to every third bit: one axis of a 30-bit Morton code
+__device__ __forceinline__ uint32_t expand_bits10(uint32_t v) {
+  v = (v * 0x00010001u) & 0xFF0000FFu;
+  v = (v * 0x00000101u) & 0x0F00F00Fu;
+  v = (v * 0x00000011u) & 0xC30C30C3u;
+  v = (v * 0x00000005u) & 0x49249249u;
+  return v;
+}
 
 // Per-point outputs of the fused KNN + mesh-distance kernel, structure-of-arrays with stride `stride`
 // (element (k, p) at [k * stride + p]) so that a warp of consecutive points reads/writes coalesced.

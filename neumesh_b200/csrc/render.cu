@@ -23,13 +23,6 @@ __device__ __forceinline__ float sigmoid_t(float x) { return __fdiv_rn(1.0f, __f
 // Spatial sort key of a ray: 30-bit Morton code of its closest point to the origin (the scene centre).  Rays are
 // rendered in key order so that the 32 rays of a warp form a compact patch: their octree walks then share nodes
 // (coalesced loads) and hit / miss rays are not mixed inside a warp.  Outputs are written back in caller order.
-__device__ __forceinline__ uint32_t spread10(uint32_t v) {
-  v = (v * 0x00010001u) & 0xFF0000FFu;
-  v = (v * 0x00000101u) & 0x0F00F00Fu;
-  v = (v * 0x00000011u) & 0xC30C30C3u;
-  v = (v * 0x00000005u) & 0x49249249u;
-  return v;
-}
 __global__ void ray_key_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d, int64_t N,
                                float radius, uint32_t* __restrict__ key, int32_t* __restrict__ idx) {
   const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -48,7 +41,7 @@ __global__ void ray_key_kernel(const float* __restrict__ rays_o, const float* __
     v = fminf(fmaxf(v, 0.f), 1023.f);
     q[c] = (uint32_t)v;
   }
-  key[r] = (spread10(q[0]) << 2) | (spread10(q[1]) << 1) | spread10(q[2]);
+  key[r] = (expand_bits10(q[0]) << 2) | (expand_bits10(q[1]) << 1) | expand_bits10(q[2]);
   idx[r] = (int32_t)r;
 }
 
@@ -242,79 +235,23 @@ __global__ void midpoints_kernel(int64_t R, int P, const float* __restrict__ z, 
   zmid[i] = __fmul_rn(0.5f, __fadd_rn(z[i + R], z[i]));
 }
 
-// renderer.py:17-24 (sdf_to_alpha), :49-63 (alpha_to_w), :299-333 (integration, white background, normals)
-__global__ void __launch_bounds__(RT)
-composite_kernel(int64_t R, int P, float s, int white_bkgd, const float* __restrict__ sdf, const float* __restrict__ zmid,
-                 const float* __restrict__ rgb_s /*[3][(P-1)*R]*/, int64_t cstride,
-                 const float* __restrict__ nabla_s /*[3][P*R] or null*/, int64_t nstride, float* __restrict__ wbuf,
-                 const int32_t* __restrict__ perm, float* __restrict__ rgb_out, float* __restrict__ depth_out,
-                 float* __restrict__ acc_out, float* __restrict__ normals_out) {
-  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (r >= R) return;
-  const int64_t dst = perm[r];   // caller's ray index
-  float c0 = sigmoid_t(__fmul_rn(sdf[r], s));
-  double T = 1.0;   // torch.cumprod on the CPU accumulates in double (see upsample_kernel)
-  float acc = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, nx = 0.f, ny = 0.f, nz = 0.f;
-  for (int j = 0; j + 1 < P; ++j) {
-    const int64_t q = (int64_t)j * R + r;
-    const float c1 = sigmoid_t(__fmul_rn(sdf[q + R], s));
-    const float alpha = fmaxf(__fdiv_rn(__fsub_rn(c0, c1), __fadd_rn(c0, 1e-10f)), 0.f);
-    const float w = __fmul_rn(alpha, (float)T);
-    T = __dmul_rn(T, (double)__fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f));
-    wbuf[q] = w;
-    acc = __fadd_rn(acc, w);
-    cr = __fadd_rn(cr, __fmul_rn(w, rgb_s[q]));
-    cg = __fadd_rn(cg, __fmul_rn(w, rgb_s[cstride + q]));
-    cb = __fadd_rn(cb, __fmul_rn(w, rgb_s[2 * cstride + q]));
-    if (nabla_s) {
-      const float gx = nabla_s[q], gy = nabla_s[nstride + q], gz = nabla_s[2 * nstride + q];
-      const float nn = fmaxf(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), __fmul_rn(gz, gz))), 1e-12f);
-      nx = __fadd_rn(nx, __fmul_rn(__fdiv_rn(gx, nn), w));
-      ny = __fadd_rn(ny, __fmul_rn(__fdiv_rn(gy, nn), w));
-      nz = __fadd_rn(nz, __fmul_rn(__fdiv_rn(gz, nn), w));
-    }
-    c0 = c1;
-  }
-  const float den = __fadd_rn(acc, 1e-10f);
-  float depth = 0.f;
-  for (int j = 0; j + 1 < P; ++j) {
-    const int64_t q = (int64_t)j * R + r;
-    depth = __fadd_rn(depth, __fmul_rn(__fdiv_rn(wbuf[q], den), zmid[q]));
-  }
-  if (white_bkgd) {
-    const float bg = __fsub_rn(1.0f, acc);
-    cr = __fadd_rn(cr, bg);
-    cg = __fadd_rn(cg, bg);
-    cb = __fadd_rn(cb, bg);
-  }
-  rgb_out[dst * 3] = cr;
-  rgb_out[dst * 3 + 1] = cg;
-  rgb_out[dst * 3 + 2] = cb;
-  depth_out[dst] = depth;
-  acc_out[dst] = acc;
-  if (normals_out) {
-    normals_out[dst * 3] = nx;
-    normals_out[dst * 3 + 1] = ny;
-    normals_out[dst * 3 + 2] = nz;
-  }
-}
-
-// ---- live-sample path (cfg.skip_dead_samples) ---------------------------------------------------------------
+// ---- compositing ---------------------------------------------------------------------------------------------
 // The reference multiplies every mid-point colour, depth and point normal by its visibility weight
 // (renderer.py:304-333).  Where that weight is exactly 0.0f - in front of the shell (sigmoid saturates to 1), behind
 // the surface (transmittance underflows), on rays that miss - the colour MLP, the mid-point nabla and the KNN walk
-// feeding them cannot influence any composited output.  The kernels below compute the weights first, compact the
-// samples with a non-zero weight and evaluate only those; the composite then adds exactly the same non-zero terms
-// in the same order, so rgb / depth / acc / normals are bit-identical to evaluating everything.
+// feeding them cannot influence any composited output.  The live-sample path (cfg.skip_dead_samples) therefore
+// computes the weights first, compacts the samples with a non-zero weight and evaluates only those; the composite
+// then adds exactly the same non-zero terms in the same order, so rgb / depth / acc / normals are bit-identical to
+// evaluating everything.  Both paths composite from the weights of weights_kernel.
 
-// pass 1 of the compositing: weights (same arithmetic as composite_kernel) + number of live samples per ray
+// renderer.py:17-24 (sdf_to_alpha), :49-63 (alpha_to_w): weights + number of live (non-zero weight) samples per ray
 __global__ void __launch_bounds__(RT)
 weights_kernel(int64_t R, int P, float s, const float* __restrict__ sdf, float* __restrict__ wbuf,
                int32_t* __restrict__ nlive) {
   const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (r >= R) return;
   float c0 = sigmoid_t(__fmul_rn(sdf[r], s));
-  double T = 1.0;   // as composite_kernel
+  double T = 1.0;   // torch.cumprod on the CPU accumulates in double (see upsample_kernel)
   int n = 0;
   for (int j = 0; j + 1 < P; ++j) {
     const int64_t q = (int64_t)j * R + r;
@@ -363,33 +300,37 @@ compact_live_kernel(int64_t R, int P, const int32_t* __restrict__ off, const flo
   }
 }
 
-// pass 2 of the compositing over the live samples only (same operation order as composite_kernel)
+// renderer.py:299-333 (integration, white background, normals) from the weights of weights_kernel.
+// off == nullptr: every sample adds its term, as the reference does (0 * NaN stays NaN); colour and nabla of mid-point
+//   j are read sample-major at [c * stride + j * R + r].
+// off != nullptr (live path): only the terms with a non-zero weight; colour and nabla of the i-th live sample of ray r
+//   are read from the compacted list at [c * stride + off[r] + i].
 __global__ void __launch_bounds__(RT)
-composite_live_kernel(int64_t R, int P, int white_bkgd, const float* __restrict__ wbuf, const float* __restrict__ zmid,
-                      const int32_t* __restrict__ off, const float* __restrict__ rgb_l /*[3][M]*/, int64_t M,
-                      const float* __restrict__ nabla_l /*[3][Mn] or null*/, int64_t Mn, const int32_t* __restrict__ perm,
-                      float* __restrict__ rgb_out, float* __restrict__ depth_out, float* __restrict__ acc_out,
-                      float* __restrict__ normals_out) {
+composite_kernel(int64_t R, int P, int white_bkgd, const float* __restrict__ wbuf, const float* __restrict__ zmid,
+                 const int32_t* __restrict__ off, const float* __restrict__ rgb /*[3][cstride]*/, int64_t cstride,
+                 const float* __restrict__ nabla /*[3][nstride] or null*/, int64_t nstride,
+                 const int32_t* __restrict__ perm, float* __restrict__ rgb_out, float* __restrict__ depth_out,
+                 float* __restrict__ acc_out, float* __restrict__ normals_out) {
   const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (r >= R) return;
-  const int64_t dst = perm[r];
+  const int64_t dst = perm[r];   // caller's ray index
   float acc = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, nx = 0.f, ny = 0.f, nz = 0.f;
-  int64_t k = off[r];
+  int64_t k = off ? off[r] : 0;  // next live-list entry
   for (int j = 0; j + 1 < P; ++j) {
-    const float w = wbuf[(int64_t)j * R + r];
-    if (w != 0.f) {
-      acc = __fadd_rn(acc, w);
-      cr = __fadd_rn(cr, __fmul_rn(w, rgb_l[k]));
-      cg = __fadd_rn(cg, __fmul_rn(w, rgb_l[M + k]));
-      cb = __fadd_rn(cb, __fmul_rn(w, rgb_l[2 * M + k]));
-      if (nabla_l) {
-        const float gx = nabla_l[k], gy = nabla_l[Mn + k], gz = nabla_l[2 * Mn + k];
-        const float nn = fmaxf(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), __fmul_rn(gz, gz))), 1e-12f);
-        nx = __fadd_rn(nx, __fmul_rn(__fdiv_rn(gx, nn), w));
-        ny = __fadd_rn(ny, __fmul_rn(__fdiv_rn(gy, nn), w));
-        nz = __fadd_rn(nz, __fmul_rn(__fdiv_rn(gz, nn), w));
-      }
-      ++k;
+    const int64_t q = (int64_t)j * R + r;
+    const float w = wbuf[q];
+    if (off && w == 0.f) continue;
+    const int64_t i = off ? k++ : q;
+    acc = __fadd_rn(acc, w);
+    cr = __fadd_rn(cr, __fmul_rn(w, rgb[i]));
+    cg = __fadd_rn(cg, __fmul_rn(w, rgb[cstride + i]));
+    cb = __fadd_rn(cb, __fmul_rn(w, rgb[2 * cstride + i]));
+    if (nabla) {
+      const float gx = nabla[i], gy = nabla[nstride + i], gz = nabla[2 * nstride + i];
+      const float nn = fmaxf(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), __fmul_rn(gz, gz))), 1e-12f);
+      nx = __fadd_rn(nx, __fmul_rn(__fdiv_rn(gx, nn), w));
+      ny = __fadd_rn(ny, __fmul_rn(__fdiv_rn(gy, nn), w));
+      nz = __fadd_rn(nz, __fmul_rn(__fdiv_rn(gz, nn), w));
     }
   }
   const float den = __fadd_rn(acc, 1e-10f);
@@ -397,7 +338,7 @@ composite_live_kernel(int64_t R, int P, int white_bkgd, const float* __restrict_
   for (int j = 0; j + 1 < P; ++j) {
     const int64_t q = (int64_t)j * R + r;
     const float w = wbuf[q];
-    if (w != 0.f) depth = __fadd_rn(depth, __fmul_rn(__fdiv_rn(w, den), zmid[q]));
+    if (!off || w != 0.f) depth = __fadd_rn(depth, __fmul_rn(__fdiv_rn(w, den), zmid[q]));
   }
   if (white_bkgd) {
     const float bg = __fsub_rn(1.0f, acc);
@@ -619,6 +560,221 @@ int64_t nmb_render_edit_workspace_bytes(const nmb_render_cfg* cfg, const nmb_edi
 
 }  // extern "C"
 
+namespace {
+
+using namespace nmb;
+
+// What every stage of a chunk reads.  The chunk's rays are perm[0..R): chunk-local ray r is the caller's ray perm[r].
+struct Chunk {
+  const nmb_field* f;
+  const nmb_edit* edit;      // nullable
+  const nmb_render_cfg* cfg;
+  int64_t N;                 // rays of the call (columns of cfg->perturb_u)
+  int64_t R;
+  int P, n_new;
+  const int32_t* perm;
+  Workspace w;
+  EditScratch es;
+  cudaStream_t stream;
+  unsigned rb;               // blocks of the per-ray kernels
+};
+
+// rays -> origin, direction, near / far (renderer.py:150-191): sphere, [bounded mesh-distance scan], [bypass]
+int setup_rays(const Chunk& c, const float* rays_o, const float* rays_d) {
+  const nmb_render_cfg* cfg = c.cfg;
+  const Workspace& w = c.w;
+  ray_setup_kernel<<<c.rb, RT, 0, c.stream>>>(rays_o, rays_d, c.perm, c.R, cfg->obj_bounding_radius,
+                                              cfg->normalize_dirs, w.orig, w.dirs, w.near, w.far, w.bnear, w.bfar);
+  NMB_LAUNCH_OK();
+  if (cfg->bounded_near_far) {
+    ShellGrid shell{};
+    if (c.R >= 65536) {   // the certificate costs ~0.1-0.3 s to build: only worth it for frame-sized renders
+      int rc = ensure_shell_grid(c.f, c.stream);
+      if (rc) return rc;
+      shell = c.f->shell;
+    }
+    int rc = launch_bound_scan(c.f->grid, c.f->indicator.p, c.f->w1, w.orig, w.dirs, w.near, w.far, c.R, 256, 0.1f,
+                               w.bnear, w.bfar, shell, c.stream);
+    if (rc) return rc;
+    bound_finish_kernel<<<c.rb, RT, 0, c.stream>>>(c.R, w.bnear, w.bfar, w.near, w.far);
+    NMB_LAUNCH_OK();
+  }
+  if (cfg->use_near_bypass || cfg->use_far_bypass) {
+    bypass_kernel<<<c.rb, RT, 0, c.stream>>>(c.R, cfg->use_near_bypass, cfg->near_bypass, cfg->use_far_bypass,
+                                             cfg->far_bypass, w.near, w.far);
+    NMB_LAUNCH_OK();
+  }
+  return 0;
+}
+
+// The field at n points whose neighbours `in` describes: sdf, and nabla where non-null; with colour also the colour
+// MLP and the edit's blend, into w.rgb ([3][in.stride] SoA) at the view directions in.dirs or in.rays_d.
+int eval_field(const Chunk& c, FieldIn in, int64_t n, float* sdf, float* nabla, bool color) {
+  int rc = launch_geo(c.f, in, n, sdf, nabla, c.stream);
+  if (rc || !color) return rc;
+  in.nabla = nabla;
+  rc = launch_color(c.f, in, n, c.w.rgb, c.stream);
+  if (rc || !c.edit) return rc;
+  return apply_edit(c.edit, in, n, c.w.rgb, c.es, c.stream);
+}
+
+// The field at S samples z [S][R] of every ray.  Their neighbours are stored as pass entries entry0.. of the
+// neighbour arrays (entry e of ray r at position e * R + r).
+int eval_samples(const Chunk& c, const float* z, int S, float* sdf, float* nabla, bool color, int64_t entry0) {
+  const Workspace& w = c.w;
+  const int64_t o = entry0 * c.R;   // first position of this pass in the neighbour arrays
+  KnnOut ko{w.k_ds + o, w.k_slot + o, w.k_w + o, w.k_grad + o, (int64_t)c.P * c.R};
+  PointSrc src{nullptr, w.orig, w.dirs, z, c.R};
+  if (entry0 > 0) {
+    // an up-sampling pass: the first new sample of a ray (u = 0 reproduces the ray's first sample exactly) starts
+    // from the stored neighbours of the ray's current first sample instead of a cold walk
+    src.seed_slot = w.k_slot;
+    src.seed_entry = w.origin;        // row 0 of origin: pass entry of sample 0 of every ray
+    src.seed_stride = (int64_t)c.P * c.R;
+  }
+  int rc = launch_knn_distance(c.f->grid, c.f->indicator.p, c.f->w1, src, (int64_t)S * c.R, ko, c.stream);
+  if (rc) return rc;
+  FieldIn in(ko);
+  in.rays_d = w.dirs;
+  in.R = c.R;
+  return eval_field(c, in, (int64_t)S * c.R, sdf, nabla, color);
+}
+
+// The sampling cascade (renderer.py:193-259): coarse samples, then N_upsample_iters x {inverse-cdf samples -> sdf ->
+// merge}.  Leaves the P sorted depths and their sdf in w.z / w.sdf, and the nabla at them in nab_pts if non-null.
+int sample_cascade(const Chunk& c, float* nab_pts) {
+  const Workspace& w = c.w;
+  const int64_t R = c.R;
+  int n = c.cfg->N_samples;
+  // The live path with normals needs sdf' and the neighbours of its live sample points again at the end.  Every pass
+  // therefore leaves its KNN results in place (coarse samples are entries 0..N_samples-1, iteration `it` adds
+  // N_samples + it * n_new ...) and an `origin` index is carried through the merges, so that pass GATHERS instead of
+  // walking the octree again (cheap: pointer offsets + one int32 per sample through the merges).
+  coarse_z_kernel<<<(unsigned)ceil_div(R * n, 256), 256, 0, c.stream>>>(R, n, w.near, w.far, w.z, w.origin);
+  NMB_LAUNCH_OK();
+  // The reference evaluates the P final samples a second time (renderer.py:271-274: forward_with_nablas when
+  // calc_normal, forward_density_only otherwise).  They are the very points of the coarse / up-sampling passes, so
+  // their sdf is already known (same point, same kernel => same bits) and the nabla, when carried, is obtained in
+  // those passes too (tangent rows) and carried through the merges: no second KNN walk, no second MLP pass.
+  float* nab_new = nab_pts ? w.nabla_mid : nullptr;   // free until the mid-point pass
+  int rc = eval_samples(c, w.z, n, w.sdf, nab_pts, false, 0);
+  if (rc) return rc;
+  const float* u = c.cfg->perturb_u;
+  for (int it = 0; it < c.cfg->N_upsample_iters; ++it) {
+    upsample_kernel<<<c.rb, RT, 0, c.stream>>>(R, n, c.n_new, 256.0f * (float)(1 << it), w.z, w.sdf, w.wbuf, w.znew,
+                                               u ? u + (int64_t)it * c.n_new * c.N : nullptr, c.N, c.perm);
+    NMB_LAUNCH_OK();
+    // deterministic up-sampling: u_0 = 0 returns the ray's first sample again, bit for bit (upsample_kernel: j = 0,
+    // denom -> 1, t = 0) - the same point through the same kernels gives the same sdf, so it is not evaluated twice
+    const int dup0 = (u == nullptr && c.n_new > 1) ? 1 : 0;
+    rc = eval_samples(c, w.znew + dup0 * R, c.n_new - dup0, w.sdfnew + dup0 * R, nab_new ? nab_new + dup0 * R : nullptr,
+                      false, n + dup0);
+    if (rc) return rc;
+    merge_kernel<<<c.rb, RT, 0, c.stream>>>(R, n, c.n_new, w.z, w.sdf, w.znew, w.sdfnew, nab_pts, nab_new,
+                                            (int64_t)c.P * R, w.origin, n, dup0);
+    NMB_LAUNCH_OK();
+    n += c.n_new;
+  }
+  return 0;
+}
+
+// Live path: compact the mid-points with a non-zero weight (*M of them) and evaluate only those; with normals also
+// the nabla at the live sample points, into w.nabla_pts.
+int eval_live(const Chunk& c, float* mid_nabla, int64_t* M) {
+  const Workspace& w = c.w;
+  const int64_t R = c.R;
+  size_t need = 0;
+  NMB_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, need, w.nlive, w.live_off, (int)R, c.stream));
+  NMB_CHECK((int64_t)need <= w.scan_bytes, "scan scratch too small");
+  size_t sb = (size_t)w.scan_bytes;
+  NMB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.scan_tmp, sb, w.nlive, w.live_off, (int)R, c.stream));
+  count_launch(2);
+  int32_t last_off = 0, last_n = 0;   // the live count sizes every launch below
+  NMB_CUDA_OK(cudaMemcpyAsync(&last_off, w.live_off + (R - 1), 4, cudaMemcpyDeviceToHost, c.stream));
+  NMB_CUDA_OK(cudaMemcpyAsync(&last_n, w.nlive + (R - 1), 4, cudaMemcpyDeviceToHost, c.stream));
+  NMB_CUDA_OK(cudaStreamSynchronize(c.stream));
+  *M = (int64_t)last_off + last_n;
+  if (*M == 0) return 0;
+  const bool normals = c.cfg->calc_normal;
+  compact_live_kernel<<<c.rb, RT, 0, c.stream>>>(R, c.P, w.live_off, w.wbuf, w.z, w.zmid, w.orig, w.dirs, w.live_mid,
+                                                 w.live_dir, nullptr, normals ? w.origin : nullptr,
+                                                 normals ? w.live_src : nullptr);
+  NMB_LAUNCH_OK();
+  if (normals) {
+    // sdf' * grad ds at the live sample POINTS, from the neighbours the sampling passes found (no second walk);
+    // must run before the mid-point pass below re-uses the neighbour arrays
+    FieldIn in(KnnOut{w.k_ds, w.k_slot, w.k_w, w.k_grad, (int64_t)c.P * R});
+    in.index = w.live_src;
+    int rc = eval_field(c, in, *M, w.sdf_mid, w.nabla_pts, false);
+    if (rc) return rc;
+  }
+  KnnOut ko{w.k_ds, w.k_slot, w.k_w, w.k_grad, *M};
+  int rc;
+  if (R >= RAY_KERNEL_MIN_RAYS) {   // warm-started per-ray lists
+    rc = launch_knn_lists(c.f->grid, c.f->indicator.p, c.f->w1, w.live_mid, w.live_off, w.nlive, R, *M, c.P - 1, ko,
+                          c.stream);
+  } else {
+    PointSrc src{w.live_mid, nullptr, nullptr, nullptr, 0};
+    rc = launch_knn_distance(c.f->grid, c.f->indicator.p, c.f->w1, src, *M, ko, c.stream);
+  }
+  if (rc) return rc;
+  FieldIn in(ko);
+  in.dirs = w.live_dir;
+  return eval_field(c, in, *M, w.sdf_mid, mid_nabla, true);
+}
+
+// Mid-points, visibility weights, colour at the mid-points (every one, or the live ones only) and the composite into
+// the caller's per-ray outputs.
+int shade(const Chunk& c, bool live, float* rgb, float* depth, float* acc, float* normals) {
+  const Workspace& w = c.w;
+  const int64_t R = c.R, PR = (int64_t)c.P * R;
+  midpoints_kernel<<<(unsigned)ceil_div(R * (c.P - 1), 256), 256, 0, c.stream>>>(R, c.P, w.z, w.zmid);
+  NMB_LAUNCH_OK();
+  weights_kernel<<<c.rb, RT, 0, c.stream>>>(R, c.P, c.f->s, w.sdf, w.wbuf, w.nlive);
+  NMB_LAUNCH_OK();
+  // the colour MLPs of the main model or of an edit's reference models may take the mid-point nabla as an input
+  const bool need_mid_nabla = c.f->lay.use_nabla != 0 || (c.edit && edit_needs_nabla(c.edit));
+  float* mid_nabla = need_mid_nabla ? w.nabla_mid : nullptr;
+  int64_t M = 0;   // live path: length of the compacted list, the stride of its colours
+  int rc = live ? eval_live(c, mid_nabla, &M) : eval_samples(c, w.zmid, c.P - 1, w.sdf_mid, mid_nabla, true, 0);
+  if (rc) return rc;
+  composite_kernel<<<c.rb, RT, 0, c.stream>>>(R, c.P, c.cfg->white_bkgd, w.wbuf, w.zmid, live ? w.live_off : nullptr,
+                                              w.rgb, live ? M : PR, c.cfg->calc_normal ? w.nabla_pts : nullptr, PR,
+                                              c.perm, rgb, depth, acc, normals);
+  NMB_LAUNCH_OK();
+  return 0;
+}
+
+// [S][R] chunk arrays -> the caller's per-ray detail outputs, each skipped when null.  A sampling_only render has
+// computed the samples, their sdf and near / far only, and exports only those.
+int export_detail(const Chunk& c, const nmb_render_detail* d) {
+  const Workspace& w = c.w;
+  const int P = c.P;
+  const int64_t PR = (int64_t)P * c.R;
+  auto ex = [&](float* dst, const float* src, int S, int C, int64_t cstride) -> int {
+    if (!dst) return 0;
+    export_samples_kernel<<<(unsigned)ceil_div(c.R * S * C, 256), 256, 0, c.stream>>>(c.R, S, C, src, cstride, c.perm,
+                                                                                      dst);
+    NMB_LAUNCH_OK();
+    return 0;
+  };
+  int rc;
+  if ((rc = ex(d->d_all, w.z, P, 1, 0))) return rc;
+  if ((rc = ex(d->implicit_surface, w.sdf, P, 1, 0))) return rc;
+  if (!c.cfg->sampling_only) {
+    if (c.cfg->calc_normal && (rc = ex(d->implicit_nablas, w.nabla_pts, P, 3, PR))) return rc;
+    if ((rc = ex(d->radiance, w.rgb, P - 1, 3, PR))) return rc;
+    if ((rc = ex(d->sdf_mid, w.sdf_mid, P - 1, 1, 0))) return rc;
+  }
+  if (d->near_far) {
+    export_near_far_kernel<<<c.rb, RT, 0, c.stream>>>(c.R, w.near, w.far, c.perm, d->near_far);
+    NMB_LAUNCH_OK();
+  }
+  return 0;
+}
+
+}  // namespace
+
 static int render_impl(const nmb_field* f, const nmb_edit* edit, const nmb_render_cfg* cfg, const float* rays_o,
                        const float* rays_d, int64_t N, int64_t rays_per_chunk, float* rgb, float* depth, float* acc,
                        float* normals, const nmb_render_detail* detail, void* workspace, int64_t workspace_bytes,
@@ -647,7 +803,6 @@ static int render_impl(const nmb_field* f, const nmb_edit* edit, const nmb_rende
   const int n_new = n_iters > 0 ? cfg->N_importance / n_iters : 0;
   const int P = cfg->N_samples + n_new * n_iters;
   void* ws_aligned = reinterpret_cast<void*>(align_up(reinterpret_cast<int64_t>(workspace), 256));
-  const nmb_grid* g = f->grid;
 
   // ---- render order: rays sorted by the Morton key of their closest point to the scene centre ----
   uint32_t *key_in = nullptr, *key_out = nullptr;
@@ -671,219 +826,21 @@ static int render_impl(const nmb_field* f, const nmb_edit* edit, const nmb_rende
   NMB_CUDA_OK(cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, key_in, key_out, idx_in, perm_all, (int)N, 0, 30, stream));
   count_launch(3);
 
+  // live path: only the mid-points with a non-zero weight are evaluated (per-sample detail outputs need them all)
+  const bool live = cfg->skip_dead_samples && !detail;
+  // full path with normals: the nabla at every sample is carried through the sampling passes
+  const bool carry_nabla = cfg->calc_normal && !live && !cfg->sampling_only;
   for (int64_t c0 = 0; c0 < N; c0 += rays_per_chunk) {
     const int64_t R = (N - c0 < rays_per_chunk) ? (N - c0) : rays_per_chunk;
-    Workspace w = carve(ws_aligned, R, P, n_new > 0 ? n_new : 1);
+    const Workspace w = carve(ws_aligned, R, P, n_new > 0 ? n_new : 1);
     const EditScratch es = edit ? edit_carve(static_cast<float*>(ws_aligned) + w.total, (int64_t)(P - 1) * R)
                                 : EditScratch{};
-    const int32_t* perm = perm_all + c0;   // chunk-local ray r  <->  caller's ray perm[r]
-    const float* ro = w.orig;
-    const unsigned rb = (unsigned)ceil_div(R, RT);
-    ray_setup_kernel<<<rb, RT, 0, stream>>>(rays_o, rays_d, perm, R, cfg->obj_bounding_radius, cfg->normalize_dirs,
-                                            w.orig, w.dirs, w.near, w.far, w.bnear, w.bfar);
-    NMB_LAUNCH_OK();
-    if (cfg->bounded_near_far) {
-      ShellGrid shell{};
-      if (R >= 65536) {   // the certificate costs ~0.1-0.3 s to build: only worth it for frame-sized renders
-        int rcs = ensure_shell_grid(f, stream);
-        if (rcs) return rcs;
-        shell = f->shell;
-      }
-      int rc = launch_bound_scan(g, f->indicator.p, f->w1, ro, w.dirs, w.near, w.far, R, 256, 0.1f, w.bnear, w.bfar,
-                                 shell, stream);
-      if (rc) return rc;
-      bound_finish_kernel<<<rb, RT, 0, stream>>>(R, w.bnear, w.bfar, w.near, w.far);
-      NMB_LAUNCH_OK();
-    }
-    if (cfg->use_near_bypass || cfg->use_far_bypass) {
-      bypass_kernel<<<rb, RT, 0, stream>>>(R, cfg->use_near_bypass, cfg->near_bypass, cfg->use_far_bypass,
-                                           cfg->far_bypass, w.near, w.far);
-      NMB_LAUNCH_OK();
-    }
-    int n = cfg->N_samples;
-    // Live path with normals: the sample points whose visibility weight is non-zero need sdf' and the neighbours again
-    // at the end.  Every pass therefore leaves its KNN results in place (pass entry e of ray r at position e * R + r of
-    // the SoA arrays: coarse samples are entries 0..N_samples-1, iteration `it` adds N_samples + it * n_new ...) and an
-    // `origin` index is carried through the merges, so the final pass GATHERS instead of walking the octree again.
-    // (cheap: pointer offsets + one int32 per sample through the merges)
-    coarse_z_kernel<<<(unsigned)ceil_div(R * n, 256), 256, 0, stream>>>(R, n, w.near, w.far, w.z,
-                                                                        w.origin);
-    NMB_LAUNCH_OK();
-
-    auto eval = [&](const float* zarr, int S, float* sdf_out, float* nabla_out, bool color, int64_t entry0) -> int {
-      const int64_t Pn = (int64_t)S * R;
-      const int64_t o = entry0 * R;   // first position of this pass in the neighbour arrays
-      KnnOut ko{w.k_ds + o, w.k_slot + o, w.k_w + o, w.k_grad + o, (int64_t)P * R};
-      PointSrc src{nullptr, ro, w.dirs, zarr, R};
-      if (entry0 > 0) {
-        // an up-sampling pass: the first new sample of a ray (u = 0 reproduces the ray's first sample exactly) starts
-        // from the stored neighbours of the ray's current first sample instead of a cold walk
-        src.seed_slot = w.k_slot;
-        src.seed_entry = w.origin;        // row 0 of origin: pass entry of sample 0 of every ray
-        src.seed_stride = (int64_t)P * R;
-      }
-      int rc = launch_knn_distance(g, f->indicator.p, f->w1, src, Pn, ko, stream);
-      if (rc) return rc;
-      FieldIn in{};
-      in.ds = ko.ds;
-      in.slot = ko.slot;
-      in.w = ko.w;
-      in.grad = ko.grad;
-      in.stride = ko.stride;
-      rc = launch_geo(f, in, Pn, sdf_out, nabla_out, stream);
-      if (rc) return rc;
-      if (color) {
-        in.nabla = nabla_out;
-        in.dirs = nullptr;
-        in.rays_d = w.dirs;
-        in.R = R;
-        rc = launch_color(f, in, Pn, w.rgb, stream);
-        if (rc) return rc;
-        if (edit && (rc = apply_edit(edit, in, Pn, w.rgb, es, stream))) return rc;
-      }
-      return 0;
-    };
-
-    // The reference evaluates the P final samples a second time (renderer.py:271-274: forward_with_nablas when
-    // calc_normal, forward_density_only otherwise).  They are the very points of the coarse / up-sampling passes, so
-    // their sdf is already known (same point, same kernel => same bits) and, with calc_normal, the nabla is obtained
-    // in those passes too (tangent rows) and carried through the merges: no second KNN walk, no second MLP pass.
-    const int64_t PR = (int64_t)P * R;
-    const bool live_path = cfg->skip_dead_samples && !detail;
-    // full path: nabla at every sample comes from the sampling passes; live path: only where the weight is non-zero
-    const bool carry_nabla = cfg->calc_normal && !live_path && !cfg->sampling_only;
-    float* nab_pts = carry_nabla ? w.nabla_pts : nullptr;
-    float* nab_new = carry_nabla ? w.nabla_mid : nullptr;   // free until the mid-point pass
-    int rc = eval(w.z, n, w.sdf, nab_pts, false, 0);
+    const Chunk c{f, edit, cfg, N, R, P, n_new, perm_all + c0, w, es, stream, (unsigned)ceil_div(R, RT)};
+    int rc = setup_rays(c, rays_o, rays_d);
+    if (!rc) rc = sample_cascade(c, carry_nabla ? w.nabla_pts : nullptr);
+    if (!rc && !cfg->sampling_only) rc = shade(c, live, rgb, depth, acc, normals);
+    if (!rc && detail) rc = export_detail(c, detail);
     if (rc) return rc;
-    for (int it = 0; it < n_iters; ++it) {
-      upsample_kernel<<<rb, RT, 0, stream>>>(R, n, n_new, 256.0f * (float)(1 << it), w.z, w.sdf, w.wbuf, w.znew,
-                                             cfg->perturb_u ? cfg->perturb_u + (int64_t)it * n_new * N : nullptr, N, perm);
-      NMB_LAUNCH_OK();
-      // deterministic up-sampling: u_0 = 0 returns the ray's first sample again, bit for bit (upsample_kernel: j = 0,
-      // denom -> 1, t = 0) - the same point through the same kernels gives the same sdf, so it is not evaluated twice
-      const int dup0 = (cfg->perturb_u == nullptr && n_new > 1) ? 1 : 0;
-      rc = eval(w.znew + dup0 * R, n_new - dup0, w.sdfnew + dup0 * R, nab_new ? nab_new + dup0 * R : nullptr, false,
-                n + dup0);
-      if (rc) return rc;
-      merge_kernel<<<rb, RT, 0, stream>>>(R, n, n_new, w.z, w.sdf, w.znew, w.sdfnew, nab_pts, nab_new, PR,
-                                          w.origin, n, dup0);
-      NMB_LAUNCH_OK();
-      n += n_new;
-    }
-    if (cfg->sampling_only) {
-      // the no-grad half of a training step (renderer.py:199-259): sample depths (+ their sdf, near / far) only
-      if (detail && detail->d_all) {
-        export_samples_kernel<<<(unsigned)ceil_div(R * P, 256), 256, 0, stream>>>(R, P, 1, w.z, 0, perm, detail->d_all);
-        NMB_LAUNCH_OK();
-      }
-      if (detail && detail->implicit_surface) {
-        export_samples_kernel<<<(unsigned)ceil_div(R * P, 256), 256, 0, stream>>>(R, P, 1, w.sdf, 0, perm,
-                                                                                 detail->implicit_surface);
-        NMB_LAUNCH_OK();
-      }
-      if (detail && detail->near_far) {
-        export_near_far_kernel<<<rb, RT, 0, stream>>>(R, w.near, w.far, perm, detail->near_far);
-        NMB_LAUNCH_OK();
-      }
-      continue;
-    }
-    midpoints_kernel<<<(unsigned)ceil_div(R * (P - 1), 256), 256, 0, stream>>>(R, P, w.z, w.zmid);
-    NMB_LAUNCH_OK();
-    // the colour MLPs of the main model or of an edit's reference models may take the mid-point nabla as an input
-    const bool need_mid_nabla = f->lay.use_nabla != 0 || (edit && edit_needs_nabla(edit));
-    if (live_path) {
-      // weights first, then only the samples that can contribute
-      weights_kernel<<<rb, RT, 0, stream>>>(R, P, f->s, w.sdf, w.wbuf, w.nlive);
-      NMB_LAUNCH_OK();
-      size_t need = 0;
-      NMB_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, need, w.nlive, w.live_off, (int)R, stream));
-      NMB_CHECK((int64_t)need <= w.scan_bytes, "scan scratch too small");
-      size_t sb = (size_t)w.scan_bytes;
-      NMB_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.scan_tmp, sb, w.nlive, w.live_off, (int)R, stream));
-      count_launch(2);
-      int32_t last_off = 0, last_n = 0;
-      NMB_CUDA_OK(cudaMemcpyAsync(&last_off, w.live_off + (R - 1), 4, cudaMemcpyDeviceToHost, stream));
-      NMB_CUDA_OK(cudaMemcpyAsync(&last_n, w.nlive + (R - 1), 4, cudaMemcpyDeviceToHost, stream));
-      NMB_CUDA_OK(cudaStreamSynchronize(stream));
-      const int64_t M = (int64_t)last_off + last_n;
-      if (M > 0) {
-        compact_live_kernel<<<rb, RT, 0, stream>>>(R, P, w.live_off, w.wbuf, w.z, w.zmid, w.orig, w.dirs, w.live_mid,
-                                                   w.live_dir, nullptr, cfg->calc_normal ? w.origin : nullptr,
-                                                   cfg->calc_normal ? w.live_src : nullptr);
-        NMB_LAUNCH_OK();
-        if (cfg->calc_normal) {
-          // sdf' * grad ds at the live sample POINTS, from the neighbours the sampling passes found (no second walk);
-          // must run before the mid-point pass below re-uses the neighbour arrays
-          FieldIn in{};
-          in.ds = w.k_ds;
-          in.slot = w.k_slot;
-          in.w = w.k_w;
-          in.grad = w.k_grad;
-          in.stride = PR;
-          in.index = w.live_src;
-          rc = launch_geo(f, in, M, w.sdf_mid, w.nabla_pts, stream);
-          if (rc) return rc;
-        }
-        auto eval_list = [&](const float* xyz, float* sdf_out, float* nabla_out, bool color) -> int {
-          KnnOut ko{w.k_ds, w.k_slot, w.k_w, w.k_grad, M};
-          int rc2;
-          if (R >= 32768) {   // enough rays to fill the GPU with one thread per ray: warm-started per-ray lists
-            rc2 = launch_knn_lists(g, f->indicator.p, f->w1, xyz, w.live_off, w.nlive, R, M, P - 1, ko, stream);
-          } else {
-            PointSrc src{xyz, nullptr, nullptr, nullptr, 0};
-            rc2 = launch_knn_distance(g, f->indicator.p, f->w1, src, M, ko, stream);
-          }
-          if (rc2) return rc2;
-          FieldIn in{};
-          in.ds = ko.ds;
-          in.slot = ko.slot;
-          in.w = ko.w;
-          in.grad = ko.grad;
-          in.stride = M;
-          rc2 = launch_geo(f, in, M, sdf_out, nabla_out, stream);
-          if (rc2) return rc2;
-          if (color) {
-            in.nabla = nabla_out;
-            in.dirs = w.live_dir;
-            rc2 = launch_color(f, in, M, w.rgb, stream);
-            if (rc2) return rc2;
-            if (edit && (rc2 = apply_edit(edit, in, M, w.rgb, es, stream))) return rc2;
-          }
-          return 0;
-        };
-        rc = eval_list(w.live_mid, w.sdf_mid, need_mid_nabla ? w.nabla_mid : nullptr, true);
-        if (rc) return rc;
-      }
-      composite_live_kernel<<<rb, RT, 0, stream>>>(R, P, cfg->white_bkgd, w.wbuf, w.zmid, w.live_off, w.rgb, M,
-                                                   cfg->calc_normal ? w.nabla_pts : nullptr, PR, perm, rgb, depth, acc,
-                                                   normals);
-      NMB_LAUNCH_OK();
-      continue;
-    }
-    rc = eval(w.zmid, P - 1, w.sdf_mid, need_mid_nabla ? w.nabla_mid : nullptr, true, 0);
-    if (rc) return rc;
-    composite_kernel<<<rb, RT, 0, stream>>>(R, P, f->s, cfg->white_bkgd, w.sdf, w.zmid, w.rgb, (int64_t)P * R,
-                                            cfg->calc_normal ? w.nabla_pts : nullptr, (int64_t)P * R, w.wbuf, perm,
-                                            rgb, depth, acc, normals);
-    NMB_LAUNCH_OK();
-    if (detail) {
-      auto ex = [&](float* dst, const float* src, int S, int C, int64_t cstride) -> int {
-        if (!dst) return 0;
-        export_samples_kernel<<<(unsigned)ceil_div(R * S * C, 256), 256, 0, stream>>>(R, S, C, src, cstride, perm, dst);
-        NMB_LAUNCH_OK();
-        return 0;
-      };
-      if ((rc = ex(detail->d_all, w.z, P, 1, 0))) return rc;
-      if ((rc = ex(detail->implicit_surface, w.sdf, P, 1, 0))) return rc;
-      if (cfg->calc_normal && (rc = ex(detail->implicit_nablas, w.nabla_pts, P, 3, (int64_t)P * R))) return rc;
-      if ((rc = ex(detail->radiance, w.rgb, P - 1, 3, (int64_t)P * R))) return rc;
-      if ((rc = ex(detail->sdf_mid, w.sdf_mid, P - 1, 1, 0))) return rc;
-      if (detail->near_far) {
-        export_near_far_kernel<<<rb, RT, 0, stream>>>(R, w.near, w.far, perm, detail->near_far);
-        NMB_LAUNCH_OK();
-      }
-    }
   }
   return 0;
 }

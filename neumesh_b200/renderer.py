@@ -86,6 +86,29 @@ def fused_cascade_model(model, rays_o, *, z_samples, random_color_direction, **c
     return geo if _cascade_eligible(geo, rays_o, **cascade_kwargs) else None
 
 
+# Outputs of render_fused that nmb_render writes: its rgb, depth, acc and normals arguments, then the fields of
+# nmb_render_detail in order ("density" is detail->sdf_mid: [N, P-1] and [N, P-1, 1] share one layout).
+_DETAIL_OUTPUTS = ("d_all", "implicit_surface", "implicit_nablas", "radiance", "density", "near_far")
+_KERNEL_OUTPUTS = ("rgb", "depth_volume", "mask_volume", "normals_volume") + _DETAIL_OUTPUTS
+
+
+def _fused_output_shapes(P, *, calc_normal, detailed_output, samples_output, sampling_only):
+    """Every output of ``render_fused`` with its per-ray shape, in the order returned (P samples per ray)."""
+    if sampling_only:
+        return OrderedDict(d_all=(P,), implicit_surface=(P,), near_far=(2,))
+    out = OrderedDict(rgb=(3,), depth_volume=(), mask_volume=())
+    if calc_normal:
+        out["normals_volume"] = (3,)
+    if detailed_output:
+        if calc_normal:
+            out["implicit_nablas"] = (P, 3)
+        out.update(implicit_surface=(P,), radiance=(P - 1, 3), alpha=(P - 1,), cdf=(P,), visibility_weights=(P - 1,),
+                   d_final=(P - 1,), d_all=(P,), near_far=(2,))
+        if samples_output:
+            out.update(xyz=(P - 1, 3), dirs=(P - 1, 3), density=(P - 1, 1), colors=(P - 1, 3))
+    return out
+
+
 def render_fused(rays_o, rays_d, model, *, obj_bounding_radius=1.0, calc_normal=False, white_bkgd=False,
                  near_bypass=None, far_bypass=None, N_samples=64, N_importance=64, N_upsample_iters=4,
                  bounded_near_far=True, detailed_output=False, samples_output=False, chunk=None,
@@ -103,23 +126,13 @@ def render_fused(rays_o, rays_d, model, *, obj_bounding_radius=1.0, calc_normal=
     o = rays_o.detach().reshape(-1, 3).float().contiguous()
     d = rays_d.detach().reshape(-1, 3).float().contiguous()
     N = o.shape[0]
+    P = N_samples + (N_importance if N_upsample_iters > 0 else 0)
+    shapes = _fused_output_shapes(P, calc_normal=calc_normal, detailed_output=detailed_output,
+                                  samples_output=samples_output, sampling_only=sampling_only)
     if N == 0:
         # an empty shard (multi-GPU renders of fewer than 128 * world rays leave some ranks without rays): same keys,
         # empty tensors, no library call (empty tensors have null data pointers)
-        P = N_samples + (N_importance if N_upsample_iters > 0 else 0)
-        out = OrderedDict([("rgb", o.new_zeros(0, 3)), ("depth_volume", o.new_zeros(0)), ("mask_volume", o.new_zeros(0))])
-        if calc_normal:
-            out["normals_volume"] = o.new_zeros(0, 3)
-        if detailed_output:
-            if calc_normal:
-                out["implicit_nablas"] = o.new_zeros(0, P, 3)
-            out.update(implicit_surface=o.new_zeros(0, P), radiance=o.new_zeros(0, P - 1, 3), alpha=o.new_zeros(0, P - 1),
-                       cdf=o.new_zeros(0, P), visibility_weights=o.new_zeros(0, P - 1), d_final=o.new_zeros(0, P - 1),
-                       d_all=o.new_zeros(0, P), near_far=o.new_zeros(0, 2))
-            if samples_output:
-                out.update(xyz=o.new_zeros(0, P - 1, 3), dirs=o.new_zeros(0, P - 1, 3), density=o.new_zeros(0, P - 1, 1),
-                           colors=o.new_zeros(0, P - 1, 3))
-        return out
+        return OrderedDict((k, o.new_zeros(0, *s)) for k, s in shapes.items())
     u_dev = None
     if (perturb or perturb_u is not None) and N_upsample_iters > 0:
         n_new = N_importance // N_upsample_iters
@@ -153,58 +166,26 @@ def render_fused(rays_o, rays_d, model, *, obj_bounding_radius=1.0, calc_normal=
         chunk = int(min(chunk, max(int(min_chunk), int(0.5 * free / per_ray))))
     nbytes = L.nmb_render_edit_workspace_bytes(C.byref(cfg), edit, chunk)
     ws = _workspace(dev, nbytes)
-    P = N_samples + (N_importance if N_upsample_iters > 0 else 0)
-    if sampling_only:
-        out = OrderedDict([("d_all", torch.empty(N, P, device=dev)), ("implicit_surface", torch.empty(N, P, device=dev)),
-                           ("near_far", torch.empty(N, 2, device=dev))])
-        det = _lib.RenderDetail(out["d_all"].data_ptr(), out["implicit_surface"].data_ptr(), None, None, None,
-                                out["near_far"].data_ptr())
-        with torch.cuda.device(dev):
-            _lib.check(L.nmb_render(field, C.byref(cfg), _lib.ptr(o), _lib.ptr(d), N, chunk, None, None, None, None,
-                                    C.byref(det), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)))
-        return out
-    rgb = torch.empty(N, 3, device=dev)
-    depth = torch.empty(N, device=dev)
-    acc = torch.empty(N, device=dev)
-    normals = torch.empty(N, 3, device=dev) if calc_normal else None
-    det, det_t = None, {}
-    if detailed_output:
-        det_t = {"d_all": torch.empty(N, P, device=dev), "implicit_surface": torch.empty(N, P, device=dev),
-                 "radiance": torch.empty(N, P - 1, 3, device=dev), "sdf_mid": torch.empty(N, P - 1, device=dev),
-                 "near_far": torch.empty(N, 2, device=dev)}
-        if calc_normal:
-            det_t["implicit_nablas"] = torch.empty(N, P, 3, device=dev)
-        det = _lib.RenderDetail(*[det_t[k].data_ptr() if k in det_t else None for k in
-                                  ("d_all", "implicit_surface", "implicit_nablas", "radiance", "sdf_mid", "near_far")])
-    args = (C.byref(cfg), _lib.ptr(o), _lib.ptr(d), N, chunk, _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(acc),
-            _lib.ptr(normals), C.byref(det) if det is not None else None, _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+    # the outputs the kernels write; the rest are recomputed from them below
+    buf = {k: o.new_empty(N, *s) for k, s in shapes.items() if k in _KERNEL_OUTPUTS}
+    det = None
+    if any(k in buf for k in _DETAIL_OUTPUTS):
+        det = _lib.RenderDetail(*[buf[k].data_ptr() if k in buf else None for k in _DETAIL_OUTPUTS])
+    args = (C.byref(cfg), _lib.ptr(o), _lib.ptr(d), N, chunk, *[_lib.ptr(buf.get(k)) for k in _KERNEL_OUTPUTS[:4]],
+            C.byref(det) if det is not None else None, _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
     with torch.cuda.device(dev):
         _lib.check(L.nmb_render(field, *args) if edit is None else L.nmb_render_edit(field, edit, *args))
-    out = OrderedDict([("rgb", rgb), ("depth_volume", depth), ("mask_volume", acc)])
-    if calc_normal:
-        out["normals_volume"] = normals
-    if detailed_output:
+    if detailed_output and not sampling_only:
         # same quantities the reference returns (renderer.py:335-348), recomputed from the exported samples
-        sdf, z = det_t["implicit_surface"], det_t["d_all"]
-        cdf = torch.sigmoid(sdf * geo.forward_s().detach())
-        alpha = ((cdf[..., :-1] - cdf[..., 1:]) / (cdf[..., :-1] + 1e-10)).clamp_min(0)
-        if calc_normal:
-            out["implicit_nablas"] = det_t["implicit_nablas"]
-        out["implicit_surface"] = sdf
-        out["radiance"] = det_t["radiance"]
-        out["alpha"] = alpha
-        out["cdf"] = cdf
-        out["visibility_weights"] = alpha_to_w(alpha)
-        out["d_final"] = 0.5 * (z[..., 1:] + z[..., :-1])
-        out["d_all"] = z
-        out["near_far"] = det_t["near_far"]
+        z = buf["d_all"]
+        buf["cdf"], buf["alpha"], buf["visibility_weights"] = sdf_to_w(buf["implicit_surface"], geo.forward_s().detach())
+        buf["d_final"] = 0.5 * (z[..., 1:] + z[..., :-1])
         if samples_output:
             dn = F.normalize(d, dim=-1) if normalize_dirs else d
-            out["xyz"] = o[:, None, :] + dn[:, None, :] * out["d_final"][..., None]
-            out["dirs"] = dn[:, None, :].expand_as(out["xyz"])
-            out["density"] = det_t["sdf_mid"][..., None]
-            out["colors"] = det_t["radiance"]
-    return out
+            buf["xyz"] = o[:, None, :] + dn[:, None, :] * buf["d_final"][..., None]
+            buf["dirs"] = dn[:, None, :].expand_as(buf["xyz"])
+            buf["colors"] = buf["radiance"]
+    return OrderedDict((k, buf[k]) for k in shapes)
 
 
 # --------------------------------------------------------------------------------------------------------------

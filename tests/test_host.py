@@ -224,6 +224,10 @@ def test_render_fused_empty_shard_needs_no_library_call():
     assert out["implicit_nablas"].shape == (0, 128, 3) and out["colors"].shape == (0, 127, 3)
     full = parallel.gather_image({k: out[k] for k in ("rgb", "depth_volume", "mask_volume", "normals_volume")}, 0, 0, 1)
     assert full["rgb"].shape == (0, 3)
+    # the sampling cascade alone (volume_render's route for texture edits and training steps) keeps its own keys
+    out = render_fused(e, e, model=None, sampling_only=True)
+    assert list(out) == ["d_all", "implicit_surface", "near_far"]
+    assert out["d_all"].shape == (0, 128) and out["implicit_surface"].shape == (0, 128) and out["near_far"].shape == (0, 2)
 
 
 def test_clock_sampler_reports_only_samples_of_the_timed_region():
