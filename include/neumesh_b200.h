@@ -46,6 +46,16 @@ int64_t nmb_alloc_count(void);
 void nmb_profile_enable(int on);
 int nmb_profile_collect(double* ms, int64_t* launches, int64_t* units, int n_classes);
 
+/* Deterministic reductions, process-wide (torch.use_deterministic_algorithms' counterpart; neumesh_b200's Python layer
+ * sets it from torch's flag before every call that reduces).  When on, the calls that sum floats across threads -
+ * nmb_tr_gemm (split-K), nmb_tr_color_out_bwd, nmb_tr_colsum, nmb_tr_geo_out_bwd, nmb_tr_input_bwd and
+ * nmb_vertex_normals - use no float atomics and no partition that depends on the GPU: their results are a function of
+ * their inputs alone, bit for bit, on any sm_90a device.  Costs stream-ordered scratch and a few extra launches (the
+ * vertex-table scatter becomes a radix sort of the (point, neighbour) entries by vertex and a segmented sum).  Off by
+ * default; reads and writes make no CUDA call. */
+void nmb_set_deterministic(int on);
+int nmb_deterministic(void);
+
 /* ---- spatial index ------------------------------------------------------------------------------------------
  * Replaces the cached grid built by MeshGrid.__init__ (models/mesh_grid.py:64-74: a V x V, K=32 FRNN self-query
  * whose only kept result is the `grid` tuple).  Builds a Morton-ordered sparse octree with tight node boxes.

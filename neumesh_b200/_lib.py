@@ -53,6 +53,8 @@ SIGNATURES = {
     "nmb_alloc_count": (_I64, []),
     "nmb_profile_enable": (None, [C.c_int]),
     "nmb_profile_collect": (C.c_int, [C.POINTER(C.c_double), C.POINTER(_I64), C.POINTER(_I64), C.c_int]),
+    "nmb_set_deterministic": (None, [C.c_int]),
+    "nmb_deterministic": (C.c_int, []),
     "nmb_grid_create": (C.c_int, [_P, _I64, _P, C.POINTER(_P)]),
     "nmb_grid_update": (C.c_int, [_P, _P, _I64, _P]),
     "nmb_grid_generation": (_I64, [_P]),
@@ -146,6 +148,20 @@ def launch_count() -> int:
 def alloc_count() -> int:
     """Device buffers the library's handles have allocated in this process (``nmb_alloc_count``)."""
     return int(lib().nmb_alloc_count())
+
+
+_deterministic = None   # the mode last given to nmb_set_deterministic from here
+
+
+def sync_deterministic():
+    """Sets the library's deterministic-reduction mode (``nmb_set_deterministic``) from
+    ``torch.are_deterministic_algorithms_enabled()`` (``warn_only=True`` counts as on).  Called before every call that
+    reduces across threads; one compare when the flag has not changed."""
+    global _deterministic
+    on = torch.are_deterministic_algorithms_enabled()
+    if on is not _deterministic:
+        lib().nmb_set_deterministic(1 if on else 0)
+        _deterministic = on
 
 
 PROFILE_CLASSES = ("knn", "bound_scan", "geo", "geo_jvp", "color", "sampler", "knn_list")

@@ -10,6 +10,8 @@ namespace nmb {
 static thread_local std::string g_error;
 static std::atomic<int64_t> g_launches{0};
 static std::atomic<int64_t> g_allocs{0};
+static std::atomic<int> g_deterministic{0};
+bool deterministic() { return g_deterministic.load(std::memory_order_relaxed) != 0; }
 void set_error(const std::string& msg) { g_error = msg; }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 void count_alloc() { g_allocs.fetch_add(1, std::memory_order_relaxed); }
@@ -105,6 +107,8 @@ int nmb_profile_collect(double* ms, int64_t* launches, int64_t* units, int n_tag
   nmb::g_recs.clear();
   return 0;
 }
+void nmb_set_deterministic(int on) { nmb::g_deterministic.store(on != 0, std::memory_order_relaxed); }
+int nmb_deterministic(void) { return nmb::deterministic() ? 1 : 0; }
 const char* nmb_last_error(void) { return nmb::g_error.c_str(); }
 int nmb_version(void) { return NMB_VERSION; }
 int64_t nmb_launch_count(void) { return nmb::g_launches.load(); }

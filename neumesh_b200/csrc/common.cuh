@@ -162,6 +162,15 @@ struct DevBuf {
 
 int sm_count();
 
+// nmb_set_deterministic's process-wide mode: the reducing launchers (csrc/train.cu, nmb_vertex_normals) then take
+// summation orders that are a function of their inputs alone (no float atomics, no partition read from sm_count()).
+bool deterministic();
+
+// cub::DeviceRadixSort::SortPairs over bits [0, end_bit) of uint32 keys with int32 values (stable: equal keys keep
+// their input order); tmp == nullptr queries tmp_bytes.  csrc/sort.cu.
+cudaError_t sort_pairs_u32(void* tmp, size_t& tmp_bytes, const uint32_t* key_in, uint32_t* key_out,
+                           const int32_t* val_in, int32_t* val_out, int n, int end_bit, cudaStream_t stream);
+
 // Optional per-kernel-class device timing (bench.py's roofline): CUDA events recorded on the launching stream
 // around the launches of one class.  Disabled by default (no events, no overhead).
 enum ProfTag { PROF_KNN = 0, PROF_BOUND = 1, PROF_GEO = 2, PROF_GEO_JVP = 3, PROF_COLOR = 4, PROF_SAMPLER = 5, PROF_KNN_LIST = 6, PROF_N = 7 };

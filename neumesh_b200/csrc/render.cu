@@ -465,6 +465,38 @@ __global__ void face_normals_kernel(const float* __restrict__ v, const int32_t* 
   }
 }
 
+// Deterministic vertex normals: the corner list (key = vertex id, value = corner 3 t + j) sorted stably by vertex; the
+// first corner of every vertex's run adds the run's face normals in triangle order.
+__global__ void corner_list_kernel(const int32_t* __restrict__ tri, int64_t n, uint32_t* __restrict__ key,
+                                   int32_t* __restrict__ corner) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  key[i] = (uint32_t)tri[i];
+  corner[i] = (int32_t)i;
+}
+
+__global__ void vertex_normal_runs_kernel(const float* __restrict__ v, const int32_t* __restrict__ tri, int64_t n,
+                                          const uint32_t* __restrict__ key, const int32_t* __restrict__ corner,
+                                          float* __restrict__ acc) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n || (i > 0 && key[i] == key[i - 1])) return;
+  float sx = 0.f, sy = 0.f, sz = 0.f;
+  for (int64_t j = i; j < n && key[j] == key[i]; ++j) {
+    const int64_t t = corner[j] / 3;
+    const int32_t a = tri[t * 3], b = tri[t * 3 + 1], c = tri[t * 3 + 2];
+    const float ax = v[a * 3], ay = v[a * 3 + 1], az = v[a * 3 + 2];
+    const float ux = v[b * 3] - ax, uy = v[b * 3 + 1] - ay, uz = v[b * 3 + 2] - az;
+    const float wx = v[c * 3] - ax, wy = v[c * 3 + 1] - ay, wz = v[c * 3 + 2] - az;
+    sx += uy * wz - uz * wy;
+    sy += uz * wx - ux * wz;
+    sz += ux * wy - uy * wx;
+  }
+  const int64_t k = key[i];
+  acc[k * 3] = sx;
+  acc[k * 3 + 1] = sy;
+  acc[k * 3 + 2] = sz;
+}
+
 __global__ void normalize_rows_kernel(float* __restrict__ n, int64_t V) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= V) return;
@@ -898,7 +930,29 @@ int nmb_vertex_normals(const float* vertices, int64_t V, const int32_t* triangle
   NMB_CHECK(vertices && triangles && normals && V > 0, "bad argument");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   NMB_CUDA_OK(cudaMemsetAsync(normals, 0, sizeof(float) * 3 * V, stream));
-  if (T > 0) {
+  if (T > 0 && nmb::deterministic()) {
+    NMB_CHECK(T < (int64_t(1) << 31) / 3 && V <= (int64_t(1) << 31), "mesh too large for the deterministic normals");
+    const int64_t n = 3 * T;
+    int bits = 1;
+    while ((int64_t(1) << bits) < V) ++bits;
+    size_t sort_bytes = 0;
+    NMB_CUDA_OK(nmb::sort_pairs_u32(nullptr, sort_bytes, nullptr, nullptr, nullptr, nullptr, (int)n, bits, stream));
+    const int64_t n_al = nmb::align_up(n, 64);
+    nmb::StreamBuf buf;   // key, key_sorted, corner, corner_sorted [3T] | sort temporaries
+    NMB_CUDA_OK(buf.alloc(4 * sizeof(uint32_t) * n_al + sort_bytes, stream));
+    uint32_t* key = buf.as<uint32_t>();
+    uint32_t* key_sorted = key + n_al;
+    int32_t* corner = reinterpret_cast<int32_t*>(key_sorted + n_al);
+    int32_t* corner_sorted = corner + n_al;
+    nmb::corner_list_kernel<<<(unsigned)nmb::ceil_div(n, 256), 256, 0, stream>>>(triangles, n, key, corner);
+    NMB_LAUNCH_OK();
+    NMB_CUDA_OK(nmb::sort_pairs_u32(corner_sorted + n_al, sort_bytes, key, key_sorted, corner, corner_sorted, (int)n,
+                                    bits, stream));
+    nmb::count_launch();
+    nmb::vertex_normal_runs_kernel<<<(unsigned)nmb::ceil_div(n, 256), 256, 0, stream>>>(vertices, triangles, n,
+                                                                                       key_sorted, corner_sorted, normals);
+    NMB_LAUNCH_OK();
+  } else if (T > 0) {
     nmb::face_normals_kernel<<<(unsigned)nmb::ceil_div(T, 256), 256, 0, stream>>>(vertices, triangles, T, normals);
     NMB_LAUNCH_OK();
   }

@@ -502,11 +502,13 @@ def pack_bgr8(rgb, H=None, W=None):
 
 
 def vertex_normals(vertices, triangles):
-    """CUDA ``nmb_vertex_normals``: area-weighted vertex normals (Open3D ``compute_vertex_normals`` semantics)."""
+    """CUDA ``nmb_vertex_normals``: area-weighted vertex normals (Open3D ``compute_vertex_normals`` semantics); bit-
+    reproducible under ``torch.use_deterministic_algorithms(True)``."""
     _lib.require_cuda(vertices, "vertex_normals")
     v = vertices.detach().float().contiguous()
     t = triangles.detach().to(torch.int32).contiguous()
     out = torch.empty_like(v)
+    _lib.sync_deterministic()
     with torch.cuda.device(v.device):
         _lib.check(_lib.lib().nmb_vertex_normals(_lib.ptr(v), v.shape[0], _lib.ptr(t), t.shape[0], _lib.ptr(out),
                                                  _lib.stream_ptr(v.device)))

@@ -7,7 +7,9 @@ colour losses back-propagate through it (a double backward through the geometry 
 * ``field_forward`` / ``field_backward`` sequence the ``nmb_tr_*`` kernels (``csrc/train.cu``): gather + blend +
   encodings, value AND forward-mode tangent rows through the softplus MLP (the tangent chain makes the nabla an ordinary
   output, so its backward is a first-order reverse pass - derivation and float64 check: ``tools/train_math_proto.py``),
-  colour MLP, and the reverse pass with split-K weight-gradient GEMMs and atomic scatter-adds into the vertex tables;
+  colour MLP, and the reverse pass with split-K weight-gradient GEMMs and atomic scatter-adds into the vertex tables
+  (under ``torch.use_deterministic_algorithms(True)``: a sorted, segmented scatter and fixed reduction orders, so that
+  the gradients are bit-reproducible);
 * ``FusedFieldFn`` wraps them in a ``torch.autograd.Function``; weight normalisation (``g * v / |v|``) stays in torch
   ops around it (a [256, K] element-wise op per layer), so ``weight_g`` / ``weight_v`` receive their gradients through
   the ordinary graph.
@@ -55,7 +57,8 @@ class FieldSpec:
 
 
 class CudaPrims:
-    """The ``nmb_tr_*`` kernels on the current CUDA stream of the tensors' device."""
+    """The ``nmb_tr_*`` kernels on the current CUDA stream of the tensors' device.  The calls that reduce across threads
+    first set the library's deterministic mode from ``torch.are_deterministic_algorithms_enabled()``."""
 
     def __init__(self, device):
         self.dev = torch.device(device)
@@ -72,6 +75,7 @@ class CudaPrims:
 
     def gemm(self, A, lda, a_kc, B, ldb, b_kc, Cm, ldc, M, N, K, bias=None, epilogue=0, mask=None, ldmask=0,
              accumulate=False):
+        _lib.sync_deterministic()
         with torch.cuda.device(self.dev):
             _lib.check(self.L.nmb_tr_gemm(_lib.ptr(A), lda, int(a_kc), _lib.ptr(B), ldb, int(b_kc), _lib.ptr(Cm), ldc,
                                           M, N, K, _lib.ptr(bias), epilogue, _lib.ptr(mask), ldmask, int(accumulate),
@@ -115,16 +119,19 @@ class CudaPrims:
                                                    _lib.ptr(rgb), self._s()))
 
     def color_out_bwd(self, b_rgb, rgb, c, w_out, bz, dw_out, db_out):
+        _lib.sync_deterministic()
         with torch.cuda.device(self.dev):
             _lib.check(self.L.nmb_tr_color_out_bwd(_lib.ptr(b_rgb), _lib.ptr(rgb), _lib.ptr(c), _lib.ptr(w_out),
                                                    c.shape[0], c.shape[1], _lib.ptr(bz), _lib.ptr(dw_out),
                                                    _lib.ptr(db_out), self._s()))
 
     def colsum(self, X, out):
+        _lib.sync_deterministic()
         with torch.cuda.device(self.dev):
             _lib.check(self.L.nmb_tr_colsum(_lib.ptr(X), X.shape[1], X.shape[0], X.shape[1], _lib.ptr(out), self._s()))
 
     def geo_out_bwd(self, b_sdf, b_nabla, bXc, G, g, h, t, w_out, bh, bt, b_G, dw_out, db_out):
+        _lib.sync_deterministic()
         with torch.cuda.device(self.dev):
             _lib.check(self.L.nmb_tr_geo_out_bwd(_lib.ptr(b_sdf), _lib.ptr(b_nabla), _lib.ptr(bXc),
                                                  bXc.shape[1] if bXc is not None else 0, _lib.ptr(G), _lib.ptr(g),
@@ -133,6 +140,7 @@ class CudaPrims:
                                                  _lib.ptr(db_out), self._s()))
 
     def input_bwd(self, spec, t, bXg, bT0, bXc, b_G, d_fg, d_fc, d_ind, d_w1):
+        _lib.sync_deterministic()
         with torch.cuda.device(self.dev):
             _lib.check(self.L.nmb_tr_input_bwd(C.byref(self._inputs(spec, t)), _lib.ptr(bXg), bXg.shape[1], _lib.ptr(bT0),
                                                bT0.shape[1], _lib.ptr(bXc), bXc.shape[1], _lib.ptr(b_G), _lib.ptr(d_fg),
