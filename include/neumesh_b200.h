@@ -289,6 +289,14 @@ int nmb_tr_gemm(const float* A, int64_t lda, int a_kcontig, const float* B, int6
                 int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int epilogue, const float* mask,
                 int64_t ldmask, int accumulate, void* stream);
 
+/* nmb_tr_gemm's contract on Hopper's tensor cores (train_engine = "tf32x3"): 3xTF32 split operands
+ * (A_lo.B_hi + A_hi.B_lo + A_hi.B_hi, fp32 accumulation; about 2^-20 |A|.|B| per product beyond fp32).  Its split-K plan
+ * depends on (M, N, K) alone and partials are added in a fixed order, so results are bit-reproducible in either
+ * deterministic mode. */
+int nmb_tr_gemm_tc(const float* A, int64_t lda, int a_kcontig, const float* B, int64_t ldb, int b_kcontig, float* C,
+                   int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int epilogue, const float* mask,
+                   int64_t ldmask, int accumulate, void* stream);
+
 typedef struct nmb_tr_inputs {
   /* inputs */
   const float* xyz;                /* [M,3] */

@@ -90,6 +90,8 @@ SIGNATURES = {
     # training-path primitives (csrc/train.cu); the nmb_tr_inputs struct is bound in train_ops.TrInputs
     "nmb_tr_gemm": (C.c_int, [_P, _I64, C.c_int, _P, _I64, C.c_int, _P, _I64, _I64, _I64, _I64, _P, C.c_int, _P, _I64,
                               C.c_int, _P]),
+    "nmb_tr_gemm_tc": (C.c_int, [_P, _I64, C.c_int, _P, _I64, C.c_int, _P, _I64, _I64, _I64, _I64, _P, C.c_int, _P,
+                                 _I64, C.c_int, _P]),
     "nmb_tr_prep": (C.c_int, [_P, _P]),
     "nmb_tr_softplus_fwd": (C.c_int, [_P, _P, _P, _P, _I64, _P]),
     "nmb_tr_softplus_bwd": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _P]),

@@ -17,9 +17,10 @@
 //   nmb_tr_input_bwd     per point: encodings' backward, scatter-add into geometry_features / color_features /
 //                        indicator_vector, indicator-weight gradient (backward of the mesh distance AND of its gradient)
 //
-// fp32 CUDA-core arithmetic (FFMA): a training step evaluates ~1.3e5 points (512 rays x 255 samples), ~0.5 TFLOP
-// including the backward - milliseconds - and gradients want fp32 accumulation order stability more than tensor-core
-// throughput; the rendering path (field_tc.cu) is where the tensor-core engine matters.
+// nmb_tr_gemm is fp32 CUDA-core arithmetic (FFMA), the default training engine.  A training step evaluates ~1.3e5
+// points (512 rays x 255 samples), ~0.5 TFLOP including the backward, most of it in these GEMMs; nmb_tr_gemm_tc
+// (train_tc.cu, train_engine = "tf32x3") runs the same contract on the tensor cores with 3xTF32 split operands, which
+// keep fp32's exponent range for the small upstream gradients.
 #include <math_constants.h>
 
 #include "../../include/neumesh_b200.h"
@@ -133,6 +134,15 @@ __global__ void reduce_splits_kernel(const float* __restrict__ part, int splits,
   for (int z = 0; z < splits; ++z) s += part[(int64_t)z * split_stride + (int64_t)m * ldp + n];
   float* dst = C + (int64_t)m * ldc + n;
   *dst = accumulate ? (*dst + s) : s;
+}
+
+// the split-K reduction of nmb_tr_gemm_tc (train_tc.cu): part [splits][M][N]
+int reduce_splits(const float* part, int splits, int64_t split_stride, int64_t M, int64_t N, float* C, int64_t ldc,
+                  int accumulate, cudaStream_t stream) {
+  reduce_splits_kernel<<<(unsigned)ceil_div(M * N, 256), 256, 0, stream>>>(part, splits, split_stride, (int)M, (int)N,
+                                                                         N, C, ldc, accumulate);
+  NMB_LAUNCH_OK();
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -67,7 +67,7 @@ class NeuMesh(nn.Module):
     def __init__(self, mesh_grid, D_density: int, D_color: int, W: int, geometry_dim: int, color_dim: int,
                  multires_view: int, multires_d: int, multires_fg: int, multires_ft: int, enable_nablas_input: bool,
                  input_view_dim=3, input_d_dim=1, ln_s=0.2996, speed_factor=1.0, learn_indicator_weight=True,
-                 mlp_engine: str = DEFAULT_MLP_ENGINE):
+                 mlp_engine: str = DEFAULT_MLP_ENGINE, train_engine: str = "fp32"):
         super().__init__()
         self.mesh_grid = mesh_grid
         V = mesh_grid.get_number_of_vertices()
@@ -100,12 +100,24 @@ class NeuMesh(nn.Module):
         if mlp_engine not in MLP_ENGINES:
             raise ValueError(f"mlp_engine must be one of {sorted(MLP_ENGINES)}")
         self.mlp_engine = mlp_engine
+        self.train_engine = train_engine
         self._field = None
         self._field_key = None
         self._field_check = {}        # mlp_engine -> None or the library's reason for refusing _cfg on that engine
         # grad-enabled queries on CUDA run the fused training op (train_ops.FusedFieldFn); False = torch-op path
         self.fused_train = True
         self._train_prims = None      # tests inject a torch implementation of the kernel interface here (CPU)
+
+    @property
+    def train_engine(self) -> str:
+        """GEMM engine of the fused training op: "fp32" (``nmb_tr_gemm``, the default) or "tf32x3"
+        (``nmb_tr_gemm_tc``, 3xTF32 on the tensor cores).  Not part of the ``state_dict``."""
+        return self._train_engine
+
+    @train_engine.setter
+    def train_engine(self, engine: str):
+        from . import train_ops
+        self._train_engine = train_ops.check_train_engine(engine)
 
     # ------------------------------------------------------------------------------------------------------
     # packed CUDA field
@@ -289,7 +301,8 @@ class NeuMesh(nn.Module):
         c = self._cfg
         spec = train_ops.FieldSpec(c["geometry_dim"], c["color_dim"], c["multires_d"], c["multires_fg"], c["multires_ft"],
                                    c["multires_view"], self.enable_nablas_input, c["D_density"], c["D_color"])
-        prims = self._train_prims if self._train_prims is not None else train_ops.CudaPrims(flat.device)
+        prims = (self._train_prims if self._train_prims is not None
+                 else train_ops.CudaPrims(flat.device, self.train_engine))
         params = [self.indicator_vector, w1_t, self.geometry_features, self.color_features]
         geo = self._geo_linears()
         for lin in geo[:-1]:

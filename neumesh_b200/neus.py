@@ -6,7 +6,8 @@ The trainer evaluates the teacher under ``torch.no_grad()`` at the 127 mid-point
 (``models/trainer.py:211-219``) - an 8 x 256 skip-MLP whose normals the reference obtains with ``autograd.grad``.  On CUDA
 with grad mode off that evaluation runs on this library's kernels:
 
-* every ``Linear`` is one ``nmb_tr_gemm`` (hand-written SGEMM, ``csrc/train.cu``) over FOUR stacked row blocks - the
+* every ``Linear`` is one ``nmb_tr_gemm`` (hand-written SGEMM, ``csrc/train.cu``; ``nmb_tr_gemm_tc``, 3xTF32 on the
+  tensor cores, with ``train_engine="tf32x3"``) over FOUR stacked row blocks - the
   value rows and the three forward-mode tangent rows d/dx, d/dy, d/dz (same weights, no bias) - so the normals come out
   of the same pass, with no autograd graph;
 * ``nmb_tr_softplus_fwd`` applies softplus(beta = 100) to the value rows and softplus' * (W t) to each tangent block;
@@ -41,6 +42,8 @@ def _eff_weight(layer):
 
 
 class ImplicitSurface(nn.Module):
+    train_engine = "fp32"   # GEMM engine of the fused no-grad evaluation (set through NeuS.train_engine)
+
     def __init__(self, W=256, D=8, skips=(4,), W_geo_feat=256, input_ch=3, radius_init=1.0, obj_bounding_size=2.0,
                  geometric_init=True, embed_multires=6, weight_norm=True, use_siren=False):
         super().__init__()
@@ -113,6 +116,8 @@ class ImplicitSurface(nn.Module):
 
 
 class RadianceNet(nn.Module):
+    train_engine = "fp32"
+
     def __init__(self, D=4, W=256, skips=(), W_geo_feat=256, embed_multires=6, embed_multires_view=4, use_view_dirs=True,
                  weight_norm=True, use_siren=False):
         super().__init__()
@@ -157,7 +162,7 @@ class RadianceNet(nn.Module):
 
 class NeuS(nn.Module):
     def __init__(self, variance_init=0.05, speed_factor=1.0, input_ch=3, W_geo_feat=-1, use_outside_nerf=False,
-                 obj_bounding_radius=1.0, surface_cfg=None, radiance_cfg=None):
+                 obj_bounding_radius=1.0, surface_cfg=None, radiance_cfg=None, train_engine="fp32"):
         super().__init__()
         if use_outside_nerf:
             raise NotImplementedError("the NeRF++ background of the mask-free NeuS setting is out of scope (DESIGN.md)")
@@ -168,6 +173,18 @@ class NeuS(nn.Module):
         if W_geo_feat < 0:
             W_geo_feat = self.implicit_surface.W
         self.radiance_net = RadianceNet(W_geo_feat=W_geo_feat, **(radiance_cfg or {}))
+        self.train_engine = train_engine
+
+    @property
+    def train_engine(self) -> str:
+        """GEMM engine of the fused no-grad surface and radiance evaluation: "fp32" (``nmb_tr_gemm``, the default) or
+        "tf32x3" (``nmb_tr_gemm_tc``, 3xTF32 on the tensor cores).  Not part of the ``state_dict``."""
+        return self.implicit_surface.train_engine
+
+    @train_engine.setter
+    def train_engine(self, engine: str):
+        from . import train_ops
+        self.implicit_surface.train_engine = self.radiance_net.train_engine = train_ops.check_train_engine(engine)
 
     def forward_radiance(self, x, view_dirs):
         _, nablas, feat = self.implicit_surface.forward_with_nablas(x)
@@ -213,7 +230,7 @@ def _fused_surface(surf: ImplicitSurface, x):
     lead = x.shape[:-1]
     flat = x.detach().reshape(-1, 3).float().contiguous()
     M, dev = flat.shape[0], flat.device
-    P = train_ops.CudaPrims(dev)
+    P = train_ops.CudaPrims(dev, surf.train_engine)
     L = max(surf.embed_multires, 0)
     emb, jac = _embed_with_jacobian(flat, L)                   # [M, C], [3, M, C]
     # rows [0, M): values; [M, 2M), [2M, 3M), [3M, 4M): tangents w.r.t. x, y, z
@@ -252,7 +269,7 @@ def _fused_radiance(net: RadianceNet, inp):
     lead = inp.shape[:-1]
     H = inp.detach().reshape(-1, inp.shape[-1]).float().contiguous()
     M, dev = H.shape[0], H.device
-    P = train_ops.CudaPrims(dev)
+    P = train_ops.CudaPrims(dev, net.train_engine)
     for i in range(net.D + 1):
         lin = net.layers[i]
         Wt = _eff_weight(lin).detach().float().contiguous()

@@ -56,13 +56,27 @@ class FieldSpec:
         self.Kc = self.offd + self.chd + self.chv + (1 + 2 * self.Lft) * self.Fc
 
 
+# GEMM engines of the training path: "fp32" = nmb_tr_gemm (FFMA SGEMM), "tf32x3" = nmb_tr_gemm_tc (3xTF32 split
+# operands on wgmma, about 2^-20 |A|.|B| per product beyond fp32; bit-reproducible in both deterministic modes)
+TRAIN_ENGINES = {"fp32": "nmb_tr_gemm", "tf32x3": "nmb_tr_gemm_tc"}
+DEFAULT_TRAIN_ENGINE = "fp32"
+
+
+def check_train_engine(engine):
+    if engine not in TRAIN_ENGINES:
+        raise ValueError(f"train_engine must be one of {sorted(TRAIN_ENGINES)}, got {engine!r}")
+    return engine
+
+
 class CudaPrims:
     """The ``nmb_tr_*`` kernels on the current CUDA stream of the tensors' device.  The calls that reduce across threads
-    first set the library's deterministic mode from ``torch.are_deterministic_algorithms_enabled()``."""
+    first set the library's deterministic mode from ``torch.are_deterministic_algorithms_enabled()``.  ``engine``
+    selects the GEMM (``TRAIN_ENGINES``); every other primitive is the same for both."""
 
-    def __init__(self, device):
+    def __init__(self, device, engine=DEFAULT_TRAIN_ENGINE):
         self.dev = torch.device(device)
         self.L = _lib.lib()
+        self.gemm_symbol = TRAIN_ENGINES[check_train_engine(engine)]
 
     def _s(self):
         return _lib.stream_ptr(self.dev)
@@ -77,9 +91,9 @@ class CudaPrims:
              accumulate=False):
         _lib.sync_deterministic()
         with torch.cuda.device(self.dev):
-            _lib.check(self.L.nmb_tr_gemm(_lib.ptr(A), lda, int(a_kc), _lib.ptr(B), ldb, int(b_kc), _lib.ptr(Cm), ldc,
-                                          M, N, K, _lib.ptr(bias), epilogue, _lib.ptr(mask), ldmask, int(accumulate),
-                                          self._s()))
+            _lib.check(getattr(self.L, self.gemm_symbol)(_lib.ptr(A), lda, int(a_kc), _lib.ptr(B), ldb, int(b_kc),
+                                                         _lib.ptr(Cm), ldc, M, N, K, _lib.ptr(bias), epilogue,
+                                                         _lib.ptr(mask), ldmask, int(accumulate), self._s()))
 
     def _inputs(self, spec, t):
         s = TrInputs()
