@@ -347,6 +347,22 @@ int nmb_tr_input_bwd(const nmb_tr_inputs* in, const float* bXg, int64_t ldbg, co
                      const float* bXc, int64_t ldbc, const float* b_G, float* d_geometry_features,
                      float* d_color_features, float* d_indicator_vector, float* d_indicator_weight, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * NeuS surface op (csrc/train_neus.cu; sequenced by neumesh_b200/neus_ops.py::FusedSurfaceFn with nmb_tr_gemm /
+ * nmb_tr_gemm_tc, nmb_tr_softplus_bwd and nmb_tr_colsum).  x [M,3]; PE(x) has C = 3 (1 + 2L) columns in the
+ * reference's order (x, sin(2^0 x), cos(2^0 x), ...).  One thread per output element, no atomics.
+ * --------------------------------------------------------------------------------------------------------------- */
+/* out[m*ldo + c] = PE(x_m)_c for c < C */
+int nmb_ns_pe(const float* x, int64_t M, int32_t L, float* out, int64_t ldo, void* stream);
+/* nabla [M,3] = J^T ebar, ebar [M,C], J = dPE(x)/dx (block-diagonal; sin / cos recomputed) */
+int nmb_ns_pe_jt(const float* x, int64_t M, int32_t L, const float* ebar, float* nabla, void* stream);
+/* b_e [M,C] = J b_nabla, b_nabla [M,3] */
+int nmb_ns_pe_j(const float* x, int64_t M, int32_t L, const float* b_nabla, float* b_e, void* stream);
+/* h[m*ldh + n] = softplus_100(z[m*N + n]) */
+int nmb_ns_softplus(const float* z, int64_t M, int64_t N, float* h, int64_t ldh, void* stream);
+/* out [M,N] = (g ? g : broadcast row [N]) * (z ? softplus'(z) : 1) */
+int nmb_ns_gate(const float* g, const float* row, const float* z, int64_t M, int64_t N, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,6 +101,12 @@ SIGNATURES = {
     "nmb_tr_colsum": (C.c_int, [_P, _I64, _I64, _I64, _P, _P]),
     "nmb_tr_geo_out_bwd": (C.c_int, [_P, _P, _P, _I64, _P, _P, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
     "nmb_tr_input_bwd": (C.c_int, [_P, _P, _I64, _P, _I64, _P, _I64, _P, _P, _P, _P, _P, _P]),
+    # NeuS surface op (csrc/train_neus.cu)
+    "nmb_ns_pe": (C.c_int, [_P, _I64, _I32, _P, _I64, _P]),
+    "nmb_ns_pe_jt": (C.c_int, [_P, _I64, _I32, _P, _P, _P]),
+    "nmb_ns_pe_j": (C.c_int, [_P, _I64, _I32, _P, _P, _P]),
+    "nmb_ns_softplus": (C.c_int, [_P, _I64, _I64, _P, _I64, _P]),
+    "nmb_ns_gate": (C.c_int, [_P, _P, _P, _I64, _I64, _P, _P]),
 }
 
 

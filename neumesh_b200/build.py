@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libneumesh_b200.so")
 SOURCES = ["api.cu", "grid.cu", "field.cu", "field_ffma.cu", "field_tc.cu", "render.cu", "shell.cu", "train.cu",
-           "train_tc.cu", "edit.cu", "deform.cu", "sort.cu"]
+           "train_tc.cu", "train_neus.cu", "edit.cu", "deform.cu", "sort.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr"]
 

@@ -25,6 +25,7 @@
 
 #include "../../include/neumesh_b200.h"
 #include "common.cuh"
+#include "train_common.cuh"
 
 namespace nmb {
 namespace tr {
@@ -145,27 +146,6 @@ int reduce_splits(const float* part, int splits, int64_t split_stride, int64_t M
   return 0;
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// positional encodings (models/base.py:52-70): [x, sin(2^0 x), cos(2^0 x), sin(2^1 x), cos(2^1 x), ...]; for a
-// D-vector every block spans all D components.  pe_c(x, c): component c of PE of a SCALAR (c = 0: x; c = 1 + 2b: sin;
-// c = 2 + 2b: cos), its first and second derivatives.
-// ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float pe_val(float x, int c) {
-  if (c == 0) return x;
-  const float f = (float)(1 << ((c - 1) >> 1));
-  return ((c - 1) & 1) ? cosf(x * f) : sinf(x * f);
-}
-__device__ __forceinline__ float pe_d1(float x, int c) {
-  if (c == 0) return 1.f;
-  const float f = (float)(1 << ((c - 1) >> 1));
-  return ((c - 1) & 1) ? -f * sinf(x * f) : f * cosf(x * f);
-}
-__device__ __forceinline__ float pe_d2(float x, int c) {
-  if (c == 0) return 0.f;
-  const float f = (float)(1 << ((c - 1) >> 1));
-  return ((c - 1) & 1) ? -f * f * cosf(x * f) : -f * f * sinf(x * f);
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -259,20 +239,6 @@ __global__ void __launch_bounds__(256) prep_kernel(PrepArgs a) {
     for (int blk = 0; blk < 1 + 2 * a.Lft; ++blk) xc[offt + blk * a.Fc + j] = pe_val(f, blk);
   }
   for (int c = offt + (1 + 2 * a.Lft) * a.Fc + lane; c < a.ldc; c += 32) xc[c] = 0.f;
-}
-
-// softplus(beta = 100, threshold = 20) and its derivatives (torch.nn.Softplus semantics)
-__device__ __forceinline__ void softplus_terms(float z, float& sp, float& s1, float& s2) {
-  if (z * 100.f > 20.f) {
-    sp = z;
-    s1 = 1.f;
-    s2 = 0.f;
-  } else {
-    const float e = expf(100.f * z);
-    sp = log1pf(e) * 0.01f;
-    s1 = e / (1.f + e);
-    s2 = 100.f * s1 * (1.f - s1);
-  }
 }
 
 __global__ void softplus_fwd_kernel(int64_t n, const float* __restrict__ z, const float* __restrict__ a,

@@ -2,19 +2,22 @@
 ``RadianceNet`` of ``models/base.py:139-311,363-440``): same constructor arguments, same ``state_dict`` keys, same
 method protocol (``forward``, ``forward_radiance``, ``forward_density_only``, ``forward_with_nablas``, ``forward_s``).
 
-The trainer evaluates the teacher under ``torch.no_grad()`` at the 127 mid-points of every training ray
-(``models/trainer.py:211-219``) - an 8 x 256 skip-MLP whose normals the reference obtains with ``autograd.grad``.  On CUDA
-with grad mode off that evaluation runs on this library's kernels:
+On CUDA float32 both uses of the model run on this library's kernels (``neus_ops.py``; derivation: DESIGN.md 4.6):
 
-* every ``Linear`` is one ``nmb_tr_gemm`` (hand-written SGEMM, ``csrc/train.cu``; ``nmb_tr_gemm_tc``, 3xTF32 on the
-  tensor cores, with ``train_engine="tf32x3"``) over FOUR stacked row blocks - the
-  value rows and the three forward-mode tangent rows d/dx, d/dy, d/dz (same weights, no bias) - so the normals come out
-  of the same pass, with no autograd graph;
-* ``nmb_tr_softplus_fwd`` applies softplus(beta = 100) to the value rows and softplus' * (W t) to each tangent block;
-* the radiance net runs with the fused ReLU epilogue.
+* **training** (NeuS stage 1, ``configs/neus_dtu_scan63.yaml``; grad mode on, ``fused_train`` set): the grad-enabled
+  ``ImplicitSurface.forward_with_nablas`` is ``FusedSurfaceFn`` - the value chain plus the reverse-mode adjoint of sdf, so
+  the nabla is an ordinary output and the eikonal / radiance losses need no double backward; the grad-enabled
+  ``ImplicitSurface.forward`` (``forward_density_only``) is its value-only mode; ``RadianceNet.forward`` without skips is
+  ``FusedRadianceFn``.  Weight normalisation and the skip layers' 1/sqrt(2) stay in torch around the ops;
+* **the no-grad teacher** (``models/trainer.py:211-219``: 127 mid-points per training ray): every ``Linear`` is one GEMM
+  over FOUR stacked row blocks - the value rows and the three forward-mode tangent rows d/dx, d/dy, d/dz (same weights,
+  no bias) - so the normals come out of the same pass; ``nmb_tr_softplus_fwd`` applies softplus to the value rows and
+  softplus' * (W t) to each tangent block; the radiance net runs with the fused ReLU epilogue.
 
-Grad-enabled calls (not used by the reference's trainer for the teacher) follow the torch-op path, which is also the
-specification of the fused one."""
+Every GEMM is ``nmb_tr_gemm`` (hand-written SGEMM) or, with ``train_engine="tf32x3"``, ``nmb_tr_gemm_tc`` (3xTF32 on the
+tensor cores).  The torch-op path - the specification of the fused one - serves CPU and float64 models,
+``fused_train = False``, radiance nets with skips, surfaces without a geometry feature, and an ``x`` that itself
+requires a gradient (the op gives ``x`` none)."""
 from __future__ import annotations
 
 import numpy as np
@@ -22,6 +25,7 @@ import torch
 import torch.nn as nn
 from torch import autograd
 
+from . import neus_ops, train_ops
 from .neumesh import get_embedder
 
 
@@ -42,7 +46,9 @@ def _eff_weight(layer):
 
 
 class ImplicitSurface(nn.Module):
-    train_engine = "fp32"   # GEMM engine of the fused no-grad evaluation (set through NeuS.train_engine)
+    train_engine = "fp32"   # GEMM engine of the fused evaluation (set through NeuS.train_engine)
+    fused_train = True      # grad-enabled CUDA calls run FusedSurfaceFn; False = torch-op path
+    _train_prims = None     # tests inject a torch implementation of the kernel interface here (CPU)
 
     def __init__(self, W=256, D=8, skips=(4,), W_geo_feat=256, input_ch=3, radius_init=1.0, obj_bounding_size=2.0,
                  geometric_init=True, embed_multires=6, weight_norm=True, use_siren=False):
@@ -87,6 +93,9 @@ class ImplicitSurface(nn.Module):
         self.surface_fc_layers = nn.ModuleList(layers)
 
     def forward(self, x, return_h=False):
+        if _surface_train_ok(self, x):
+            val, _, h = _train_surface(self, x, with_nabla=False)
+            return (val, h) if return_h else val
         x = self.embed_fn(x)
         h = x
         for i in range(self.D):
@@ -105,6 +114,8 @@ class ImplicitSurface(nn.Module):
         has_grad = torch.is_grad_enabled() if has_grad_bypass is None else has_grad_bypass
         if not has_grad and x.is_cuda and _fused_ok(self):
             return _fused_surface(self, x)
+        if has_grad and _surface_train_ok(self, x):
+            return _train_surface(self, x, with_nabla=True)
         with torch.enable_grad():
             x = x.requires_grad_(True)
             val, h = self.forward(x, return_h=True)
@@ -117,6 +128,8 @@ class ImplicitSurface(nn.Module):
 
 class RadianceNet(nn.Module):
     train_engine = "fp32"
+    fused_train = True      # grad-enabled CUDA calls run FusedRadianceFn; False = torch-op path
+    _train_prims = None
 
     def __init__(self, D=4, W=256, skips=(), W_geo_feat=256, embed_multires=6, embed_multires_view=4, use_view_dirs=True,
                  weight_norm=True, use_siren=False):
@@ -152,6 +165,8 @@ class RadianceNet(nn.Module):
         inp = self._input(x, view_dirs, normals, geometry_feature)
         if not torch.is_grad_enabled() and inp.is_cuda and not self.skips:
             return _fused_radiance(self, inp)
+        if not self.skips and self.W == train_ops.HIDDEN and _fused_train_ok(self, inp):
+            return _train_radiance(self, inp)
         h = inp
         for i in range(self.D + 1):
             if i in self.skips:
@@ -177,14 +192,31 @@ class NeuS(nn.Module):
 
     @property
     def train_engine(self) -> str:
-        """GEMM engine of the fused no-grad surface and radiance evaluation: "fp32" (``nmb_tr_gemm``, the default) or
-        "tf32x3" (``nmb_tr_gemm_tc``, 3xTF32 on the tensor cores).  Not part of the ``state_dict``."""
+        """GEMM engine of the fused surface and radiance evaluation (training and no-grad): "fp32" (``nmb_tr_gemm``,
+        the default) or "tf32x3" (``nmb_tr_gemm_tc``, 3xTF32 on the tensor cores).  Not part of the ``state_dict``."""
         return self.implicit_surface.train_engine
 
     @train_engine.setter
     def train_engine(self, engine: str):
-        from . import train_ops
         self.implicit_surface.train_engine = self.radiance_net.train_engine = train_ops.check_train_engine(engine)
+
+    @property
+    def fused_train(self) -> bool:
+        """Grad-enabled CUDA calls run the fused training ops (``neus_ops``); False = torch-op path.  Default True, as
+        ``NeuMesh.fused_train``; not part of the ``state_dict``."""
+        return self.implicit_surface.fused_train
+
+    @fused_train.setter
+    def fused_train(self, on: bool):
+        self.implicit_surface.fused_train = self.radiance_net.fused_train = bool(on)
+
+    @property
+    def _train_prims(self):
+        return self.implicit_surface._train_prims
+
+    @_train_prims.setter
+    def _train_prims(self, prims):
+        self.implicit_surface._train_prims = self.radiance_net._train_prims = prims
 
     def forward_radiance(self, x, view_dirs):
         _, nablas, feat = self.implicit_surface.forward_with_nablas(x)
@@ -205,11 +237,61 @@ class NeuS(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# fused no-grad evaluation on the library's kernels
+# fused evaluation on the library's kernels
 # ------------------------------------------------------------------------------------------------------------------
 def _fused_ok(surface: ImplicitSurface) -> bool:
     return surface.W_geo_feat > 0 and surface.embed_multires >= 0 and all(
         isinstance(l, nn.Linear) for l in surface.surface_fc_layers)
+
+
+def _fused_train_ok(module, *tensors) -> bool:
+    """Grad mode on, ``fused_train`` set, the inputs and parameters float32 and on CUDA (on any device when tests
+    inject ``_train_prims``)."""
+    if not (module.fused_train and torch.is_grad_enabled()):
+        return False
+    ts = list(tensors) + list(module.parameters())
+    return all(t.dtype == torch.float32 and (t.is_cuda or module._train_prims is not None) for t in ts)
+
+
+def _surface_train_ok(surf: ImplicitSurface, x) -> bool:
+    # the op gives x no gradient: an x that needs one (a graph behind it, or a leaf that requires it) keeps the torch path
+    return not x.requires_grad and _fused_ok(surf) and _fused_train_ok(surf, x)
+
+
+def _surface_params(surf: ImplicitSurface):
+    """Effective weights of the surface MLP (weight norm, the skip layers' 1/sqrt(2) folded in), differentiable."""
+    params = []
+    for i, lin in enumerate(surf.surface_fc_layers):
+        W = _eff_weight(lin)
+        if i in surf.skips:
+            W = W * (1.0 / np.sqrt(2))
+        params += [W, lin.bias]
+    return params
+
+
+def _prims(module, device):
+    return module._train_prims if module._train_prims is not None else train_ops.CudaPrims(device, module.train_engine)
+
+
+def _train_surface(surf: ImplicitSurface, x, with_nabla):
+    """-> (sdf [...], nabla [...,3] or None, feature [...,W_geo]) through FusedSurfaceFn."""
+    lead = x.shape[:-1]
+    flat = x.reshape(-1, 3)
+    res = neus_ops.FusedSurfaceFn.apply(_prims(surf, flat.device), max(surf.embed_multires, 0), tuple(surf.skips),
+                                        with_nabla, flat, *_surface_params(surf))
+    out, nabla = res if with_nabla else (res, None)
+    sdf, feat = out[:, 0].reshape(lead), out[:, 1:].reshape(*lead, out.shape[1] - 1)
+    return sdf, (nabla.reshape(*lead, 3) if with_nabla else None), feat
+
+
+def _train_radiance(net: RadianceNet, inp):
+    lead = inp.shape[:-1]
+    params = []
+    for lin in net.layers:
+        params += [_eff_weight(lin), lin.bias]
+    flat = inp.reshape(-1, inp.shape[-1])
+    rgb = neus_ops.FusedRadianceFn.apply(_prims(net, flat.device), flat, *params)
+    return rgb.reshape(*lead, 3)
 
 
 def _embed_with_jacobian(x, L):
@@ -265,7 +347,6 @@ def _fused_surface(surf: ImplicitSurface, x):
 
 
 def _fused_radiance(net: RadianceNet, inp):
-    from . import train_ops
     lead = inp.shape[:-1]
     H = inp.detach().reshape(-1, inp.shape[-1]).float().contiguous()
     M, dev = H.shape[0], H.device

@@ -160,6 +160,28 @@ class CudaPrims:
                                                bT0.shape[1], _lib.ptr(bXc), bXc.shape[1], _lib.ptr(b_G), _lib.ptr(d_fg),
                                                _lib.ptr(d_fc), _lib.ptr(d_ind), _lib.ptr(d_w1), self._s()))
 
+    # ---- NeuS surface op (csrc/train_neus.cu); strided destinations are given as a flat view from their first element
+    def pe(self, x, L, out, ldo):
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.nmb_ns_pe(_lib.ptr(x), x.shape[0], L, _lib.ptr(out), ldo, self._s()))
+
+    def pe_jt(self, x, L, ebar, nabla):
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.nmb_ns_pe_jt(_lib.ptr(x), x.shape[0], L, _lib.ptr(ebar), _lib.ptr(nabla), self._s()))
+
+    def pe_j(self, x, L, b_nabla, b_e):
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.nmb_ns_pe_j(_lib.ptr(x), x.shape[0], L, _lib.ptr(b_nabla), _lib.ptr(b_e), self._s()))
+
+    def softplus(self, z, h, ldh):
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.nmb_ns_softplus(_lib.ptr(z), z.shape[0], z.shape[1], _lib.ptr(h), ldh, self._s()))
+
+    def gate(self, g, row, z, out):
+        with torch.cuda.device(self.dev):
+            _lib.check(self.L.nmb_ns_gate(_lib.ptr(g), _lib.ptr(row), _lib.ptr(z), out.shape[0], out.shape[1],
+                                          _lib.ptr(out), self._s()))
+
 
 # ------------------------------------------------------------------------------------------------------------------
 # sequencing (shared by the CUDA primitives and the tests' torch primitives)
@@ -207,15 +229,51 @@ def field_forward(P, spec: FieldSpec, t: dict, geo, geo_out, col, col_out, with_
     P.geo_out_fwd(hs[-1], ts[-1], geo_out[0], geo_out[1], S["G"], sdf, g, nabla, S["Xc"] if spec.use_nabla else None)
     cs, rgb = [S["Xc"]], None
     if with_color:
-        for l, (W, b) in enumerate(col):
-            K = spec.Kc if l == 0 else HIDDEN
-            c = P.empty(M, HIDDEN)
-            _linear(P, cs[-1], K, W, b, c, relu=True)
-            cs.append(c)
-        rgb = P.empty(M, 3)
-        P.color_out_fwd(cs[-1], col_out[0], col_out[1], rgb)
+        rgb, cs = color_forward(P, S["Xc"], spec.Kc, col, col_out)
     S.update(hs=hs, ts=ts, zs=zs, as_=as_, cs=cs, g=g, rgb=rgb)
     return sdf, nabla, rgb, S
+
+
+def color_forward(P, X, K, col, col_out):
+    """The colour MLP (ReLU layers of width 256, then a 3-wide sigmoid) over X[:, :K] -> (rgb [M,3], activations
+    [X, c_1, ..., c_D]).  Shared by the NeuMesh field op and the NeuS radiance op."""
+    M = X.shape[0]
+    cs = [X]
+    for l, (W, b) in enumerate(col):
+        c = P.empty(M, HIDDEN)
+        _linear(P, cs[-1], K if l == 0 else HIDDEN, W, b, c, relu=True)
+        cs.append(c)
+    rgb = P.empty(M, 3)
+    P.color_out_fwd(cs[-1], col_out[0], col_out[1], rgb)
+    return rgb, cs
+
+
+def color_backward(P, cs, rgb, K, col, col_out, b_rgb, bX):
+    """Backward of ``color_forward``: -> ([(dW, db)] per layer, (dW_out, db_out)); the input gradient goes to
+    bX[:, :K] (left as it is when there is no upstream gradient)."""
+    M = cs[0].shape[0]
+    dWo, dbo = P.zeros(3, HIDDEN), P.zeros(3)
+    col_grads = [None] * len(col)
+    if b_rgb is not None and rgb is not None:
+        bz = P.empty(M, HIDDEN)
+        P.color_out_bwd(b_rgb, rgb, cs[-1], col_out[0], bz, dWo, dbo)
+        for l in reversed(range(len(col))):
+            W, _ = col[l]
+            Kl = K if l == 0 else HIDDEN
+            dW, db = P.empty(HIDDEN, W.shape[1]), P.zeros(HIDDEN)
+            _bwd_weight(P, bz, cs[l], Kl, dW, accumulate=False)
+            P.colsum(bz, db)
+            col_grads[l] = (dW, db)
+            if l > 0:
+                nxt = P.empty(M, HIDDEN)
+                _bwd_data(P, bz, W, HIDDEN, nxt, mask=cs[l])   # ReLU of the layer below
+                bz = nxt
+            else:
+                _bwd_data(P, bz, W, K, bX)
+    else:
+        for l, (W, _) in enumerate(col):
+            col_grads[l] = (P.zeros(HIDDEN, W.shape[1]), P.zeros(HIDDEN))
+    return col_grads, (dWo, dbo)
 
 
 def field_backward(P, spec: FieldSpec, S: dict, geo, geo_out, col, col_out, b_sdf, b_nabla, b_rgb, want_w1=True):
@@ -224,29 +282,8 @@ def field_backward(P, spec: FieldSpec, S: dict, geo, geo_out, col, col_out, b_sd
     M = S["xyz"].shape[0]
     out = {}
     # ---- colour MLP ----
-    dWo, dbo = P.zeros(3, HIDDEN), P.zeros(3)
-    col_grads = [None] * len(col)
     bXc = P.zeros(M, spec.Kc)
-    if b_rgb is not None and S["rgb"] is not None:
-        bz = P.empty(M, HIDDEN)
-        P.color_out_bwd(b_rgb, S["rgb"], S["cs"][-1], col_out[0], bz, dWo, dbo)
-        for l in reversed(range(len(col))):
-            W, _ = col[l]
-            K = spec.Kc if l == 0 else HIDDEN
-            dW, db = P.empty(HIDDEN, W.shape[1]), P.zeros(HIDDEN)
-            _bwd_weight(P, bz, S["cs"][l], K, dW, accumulate=False)
-            P.colsum(bz, db)
-            col_grads[l] = (dW, db)
-            if l > 0:
-                nxt = P.empty(M, HIDDEN)
-                _bwd_data(P, bz, W, HIDDEN, nxt, mask=S["cs"][l])   # ReLU of the layer below
-                bz = nxt
-            else:
-                _bwd_data(P, bz, W, spec.Kc, bXc)
-    else:
-        for l, (W, _) in enumerate(col):
-            col_grads[l] = (P.zeros(HIDDEN, W.shape[1]), P.zeros(HIDDEN))
-    out["col"], out["col_out"] = col_grads, (dWo, dbo)
+    out["col"], out["col_out"] = color_backward(P, S["cs"], S["rgb"], spec.Kc, col, col_out, b_rgb, bXc)
     # ---- geometry MLP: value and tangent chains ----
     bh, bt, b_G = P.empty(M, HIDDEN), P.empty(M, HIDDEN), P.empty(M, 3)
     dwo, dbo_g = P.zeros(1, HIDDEN), P.zeros(1)
